@@ -1,5 +1,5 @@
 /*
- * lurk_b200.h -- C ABI of liblurk_b200.so: the B200 (sm_100a) implementation of lurk-beta's Nova/SuperNova
+ * lurk_b200.h -- C ABI of liblurk_b200.so: the H100 (sm_90a) implementation of lurk-beta's Nova/SuperNova
  * proving hot path (SURVEY.md section 8).  Plain pointers and sizes only; no C++/torch types.
  *
  * The reference (argumentcomputer/lurk-beta @ f238d85c) has no FFI of its own: GPU work is delegated to

@@ -1,4 +1,4 @@
-"""lurk-beta_b200: B200 (sm_100a) implementation of lurk-beta's Nova/SuperNova proving hot path.
+"""lurk-beta_b200: H100 (sm_90a) implementation of lurk-beta's Nova/SuperNova proving hot path.
 
 Only the path of SURVEY.md section 8: Poseidon digests and slot witnesses, store-DAG hydration, the Pedersen
 commitment MSM and the fold helpers, behind the C ABI of include/lurk_b200.h (liblurk_b200.so).  This package is the

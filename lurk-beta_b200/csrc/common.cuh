@@ -78,7 +78,7 @@ inline int sm_count() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }

@@ -181,8 +181,9 @@ extern "C" int lurk_dag_hash(int field_id, const lurk_dag_node *nodes, size_t n,
 
 // Routing aid for the caller (StoreCore::hydrate_z_cache, src/lem/store_core.rs:256-269): a level of the DAG costs one
 // dependent Poseidon latency on the GPU (~170 us: three launches + one warp-per-sponge hash) whatever its width, a CPU core
-// hashes ~20 k nodes/s, and the wide-DAG GPU rate is ~23 M nodes/s (profiles/r1_ncu_summary.md).  The library never hashes on
-// the CPU itself; it tells the caller when its own CPU path is the better choice (deep, narrow stores).
+// hashes ~20 k nodes/s, and the wide-DAG GPU rate is ~23 M nodes/s (constants of an earlier GPU generation, not re-measured on
+// the H100).  The library never hashes on the CPU itself; it tells the caller when its own CPU path is the better choice (deep,
+// narrow stores).
 extern "C" int lurk_dag_hash_plan(const lurk_dag_node *nodes, size_t n, size_t n_atoms, lurk_dag_plan *plan) {
     if (!plan || (n && !nodes)) { set_error("null argument"); return LURK_ERR_ARG; }
     memset(plan, 0, sizeof *plan);

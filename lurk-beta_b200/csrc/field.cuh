@@ -1,4 +1,4 @@
-// 256-bit prime-field arithmetic in Montgomery form, 8 x 32-bit limbs, written for sm_100a.
+// 256-bit prime-field arithmetic in Montgomery form, 8 x 32-bit limbs, written for sm_90a.
 //
 // The same templates compile for the host (carry flag emulated) so that the exact algorithm that runs on
 // the GPU is unit-tested on CPU and is reused by the host-side code of the library (Poseidon constant
@@ -224,8 +224,8 @@ struct alignas(16) Fe {
         return r;
     }
 #endif
-    // A dedicated squaring (36 word products + doubling instead of 64) was measured SLOWER on B200: the extra
-    // carry/shift work lands on the ALU pipe and as IMAD.MOV on the FMA pipe (round-1 notes in DESIGN.md).
+    // No dedicated squaring (36 word products + doubling instead of 64): the extra carry/shift work lands on the ALU
+    // pipe and as IMAD.MOV on the FMA pipe, which ate the saving in an earlier measurement.
     LURK_HD Fe sqr() const { return *this * *this; }
     LURK_HD Fe pow5() const { Fe x2 = sqr(); Fe x4 = x2.sqr(); return x4 * *this; }
 

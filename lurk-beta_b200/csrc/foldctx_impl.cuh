@@ -26,8 +26,11 @@ static constexpr int FOLD_MAX_WORLD = 16;
 static constexpr int FOLD_MAX_DEPTH = 4;
 static constexpr int FOLD_MAX_SPANS = 4;
 static constexpr int FOLD_RO_RATE = 24;            // Arecibo's RO: neptune sponge over PoseidonConstants<_, U24>
-static constexpr int FOLD_W_WINDOW = 17;           // window of commit(W2 - D) (own table when narrower than the key's; measured 20 / 18 / 17: 3.90 / 3.62 / 3.56 ms per fold)
-static constexpr int FOLD_T_WINDOW = 16;           // widest window of the chain-critical commit(T) (measured: profiles/r2_ncu_summary.md)
+// Windows of the fold's own tables.  On an H100 (400 W) at fib rc = 100, W = 16 / 17 / 18 and T = 15 / 16 / 17 all land within
+// 1 % of each other (4.31-4.37 ms per fold, about the run-to-run spread); a narrower window than the key's c = 20 shortens the
+// bucket reduction on the chain.
+static constexpr int FOLD_W_WINDOW = 17;           // window of commit(W2 - D) (own table when narrower than the key's)
+static constexpr int FOLD_T_WINDOW = 16;           // widest window of the chain-critical commit(T)
 
 // ----------------------------------------------------------------------------- fold kernels (witness field)
 struct CsrDev {

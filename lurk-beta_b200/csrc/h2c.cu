@@ -5,7 +5,7 @@
 // Data flow of lurk_ck_generate_dev: the SHAKE256 stream is inherently sequential, so a host thread squeezes it in chunks of
 // 2^16 x 32 bytes into two pinned buffers while the GPU maps the previous chunk: H2D copy and kernel of chunk k run under the
 // squeeze of chunk k + 1.  The key is written where the commitment contexts read it (n x 64 bytes, Montgomery, device memory:
-// lurk_msm_ctx_create_dev) and never crosses PCIe.  One thread per point, persistent grid of 148 x 4 CTAs of 128 threads.
+// lurk_msm_ctx_create_dev) and never crosses PCIe.  One thread per point, persistent grid of 4 CTAs of 128 threads per SM.
 #include "common.cuh"
 #include "h2c_params.h"
 

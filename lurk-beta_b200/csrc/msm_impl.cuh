@@ -1,4 +1,4 @@
-// K4: Pedersen commitment = Pippenger multi-scalar multiplication on sm_100a.
+// K4: Pedersen commitment = Pippenger multi-scalar multiplication on sm_90a.
 //
 // Replaces Arecibo's CommitmentEngineTrait::commit -> DlogGroup::vartime_multiscalar_mul (third-party crate, called
 // from RecursiveSNARK::prove_step; reference call sites src/proof/nova.rs:287,292, src/proof/supernova.rs:231-244).
@@ -290,8 +290,8 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate_kernel(const uint32_
 // tail is copied), which halves every run: out run k has ceil(m_k / 2) affine points.  One or two such rounds (half resp. three
 // quarters of all additions) run before the fixed-length-segment XYZZ accumulation takes the rest.
 static constexpr int PAIR_B = 16;        // output points per thread and batch
-// default number of pair rounds for long / short average runs: 0 = off (measured slower than the plain XYZZ accumulation on
-// B200 as implemented: the per-batch inversion stalls its CTA; profiles/r2_ncu_summary.md) -- LURK_MSM_PAIR_ROUNDS overrides
+// default number of pair rounds for long / short average runs: 0 = off (one round makes the fold step slower as implemented,
+// 4.94 vs 4.34 ms on an H100 at 400 W: the per-batch inversion stalls its CTA) -- LURK_MSM_PAIR_ROUNDS overrides
 static constexpr int MSM_PAIR_ROUNDS_LONG = 0, MSM_PAIR_ROUNDS_SHORT = 0;
 
 static __global__ void __launch_bounds__(256) msm_halve_kernel(const uint32_t *__restrict__ offs_in, uint32_t nbuckets, uint32_t *__restrict__ counts_out) {

@@ -1,4 +1,4 @@
-// K1 / K3: batch Poseidon digests and slot witnesses on sm_100a.
+// K1 / K3: batch Poseidon digests and slot witnesses on sm_90a.
 //
 // Replaces (reference): PoseidonCache::hash3/4/6/8 (src/hash.rs:180-203) and the Poseidon body of
 // allocate_slot (src/lem/circuit.rs:212-315) for whole batches.  Both run Neptune's optimised round schedule

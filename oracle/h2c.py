@@ -8,7 +8,7 @@ n = next_power_of_two(max(#constraints, #variables, ck_floor)) -> `DlogGroup::fr
     reader = SHAKE256(label).xof();  uniform_i = next 32 bytes of the stream, i = 0..n-1        (sequential)
     G_i = Curve::hash_to_curve("from_uniform_bytes")(uniform_i)  -> affine                     (independent per i)
 
-Arecibo (git, branch dev), halo2curves 0.6.0 and pasta_curves 0.5.0 are NOT under /root/reference (Cargo.toml:42,68,70-73);
+Arecibo (git, branch dev), halo2curves 0.6.0 and pasta_curves 0.5.0 are NOT under the reference checkout (Cargo.toml:42,68,70-73);
 this file restates their published algorithms:
   * hash_to_field: expand_message_xmd (RFC 9380 5.3.1) with BLAKE2b-512 (hash_length 64, empty personalisation),
     len_in_bytes 128, DST = domain_prefix || "-" || curve_id || "_XMD:BLAKE2b_" || method || "_RO_"; each 64-byte half is

@@ -1,7 +1,7 @@
 """
 ORACLE (test infrastructure, NOT product code) -- the KZG side of the BN256 path (SURVEY.md 8(f) N3 / N4).
 
-Restates, from the public Arecibo crate (git, branch dev -- NOT under /root/reference; provider/hyperkzg.rs, provider/kzg_commitment.rs,
+Restates, from the public Arecibo crate (git, branch dev -- NOT under the reference checkout; provider/hyperkzg.rs, provider/kzg_commitment.rs,
 provider/non_hiding_kzg.rs), what the reference's BN256 engine (`Bn256EngineKZG` with `hyperkzg::EvaluationEngine`, reference
 src/proof/nova.rs:65-71) does with vectors:
   * key: UniversalKZGParam::gen_srs_for_testing -> powers_of_g[i] = beta^i g  (how beta and g come out of the label-seeded RNG is not

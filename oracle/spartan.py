@@ -1,7 +1,7 @@
 """
 ORACLE (test infrastructure, NOT product code) -- the verifier's side of Spartan's relaxed-R1CS argument as Arecibo's
 spartan::snark::RelaxedR1CSSNARK runs it inside `compress` (reference src/proof/nova.rs:341-373; Arecibo is not under
-/root/reference -- restated from the public crate, the transcript replaced by an explicit challenge function):
+the reference checkout -- restated from the public crate, the transcript replaced by an explicit challenge function):
 
   z = (W padded to 2^t | u | X | 0 ..) of length 2^(t+1);  rows padded to 2^s
   outer sum-check (degree 3, claim 0) of  eq(tau, x) (Az(x) Bz(x) - u Cz(x) - E(x))                      -> r_x

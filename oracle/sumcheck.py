@@ -4,7 +4,7 @@ steps (SURVEY.md 8(f) N4: `compress`, reference src/proof/nova.rs:341-356 -> Are
 spartan::snark::RelaxedR1CSSNARK::prove -> SumcheckProof::{prove_cubic_with_additive_term, prove_quad} and
 provider::ipa_pc::InnerProductArgument::prove).
 
-Arecibo (git, branch dev) is NOT under /root/reference; restated from the public crate (spartan/sumcheck.rs,
+Arecibo (git, branch dev) is NOT under the reference checkout; restated from the public crate (spartan/sumcheck.rs,
 spartan/polys/{multilinear,eq,univariate}.rs, provider/ipa_pc.rs):
   * MultilinearPolynomial: evaluations Z[0 .. 2^l) over the boolean cube, index bit l-1 (the TOP bit) = first variable;
     bind_poly_var_top(r): Z[i] <- Z[i] + r (Z[i + n/2] - Z[i]) for i < n/2, length halves.

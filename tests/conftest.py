@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # the oracle is the checker; build it if the .so is not there yet (gcc only, seconds)
     if not os.path.exists(os.path.join(ROOT, "oracle", "liboracle.so")):
         subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "oracle")])

@@ -210,7 +210,7 @@ def test_chained_commitment_goldens_through_store_flattening(HL):
 
 def test_hydration_plan_routes_chains_to_the_cpu_and_wide_dags_to_the_gpu(L):
     """lurk_dag_hash_plan (host only): a 2000-deep cons chain is one dependent hash per level -- slower on the GPU than one
-    CPU core (profiles/r1_ncu_summary.md: 337 ms vs ~100 ms) -- so the plan keeps it on the caller's CPU path; a wide store
+    CPU core -- so the plan keeps it on the caller's CPU path; a wide store
     goes to the GPU.  Malformed input is rejected as by lurk_dag_hash."""
     import ctypes as C
     import numpy as np

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Measurements of the individual BASELINE.json configurations and of the HBM-bound helper kernels (one JSON object per
-line).  bench.py stays the contract for the headline metric; this produces the per-kernel evidence kept in profiles/.
+line).  bench.py stays the contract for the headline metric; this produces the per-kernel evidence.
   single process:  python tools/config_benches.py
   N GPUs:          python -m torch.distributed.run --nproc-per-node N ... tools/config_benches.py --only msm24"""
 import argparse

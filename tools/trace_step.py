@@ -3,6 +3,7 @@ and duration, plus the union of busy intervals.  Development aid."""
 import json
 import os
 import sys
+import tempfile
 
 import torch
 from torch.profiler import ProfilerActivity, profile
@@ -23,8 +24,9 @@ with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
         wl.step(False)
     wl.drain()
     torch.cuda.synchronize()
-prof.export_chrome_trace("gpurun_out/trace.json")
-ev = json.load(open("gpurun_out/trace.json"))["traceEvents"]
+trace = os.path.join(tempfile.mkdtemp(), "trace.json")
+prof.export_chrome_trace(trace)
+ev = json.load(open(trace))["traceEvents"]
 ks = [e for e in ev if e.get("cat") in ("kernel", "gpu_memcpy", "gpu_memset") and "ts" in e]
 ks.sort(key=lambda e: e["ts"])
 t0 = ks[0]["ts"]
