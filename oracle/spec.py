@@ -379,13 +379,50 @@ def ec_add(P, Q, p):
 
 
 def ec_mul(k, P, p):
-    R = None
-    while k:
-        if k & 1:
-            R = ec_add(R, P, p)
-        P = ec_add(P, P, p)
-        k >>= 1
-    return R
+    """k P on y^2 = x^3 + b (a = 0): double-and-add in Jacobian coordinates, one inversion at the end"""
+    if P is None or k == 0:
+        return None
+    x2, y2 = P
+    X, Y, Z = 1, 1, 0                       # the identity
+    for bit in bin(k)[2:]:
+        if Z:                               # doubling (dbl-2009-l)
+            A, B = X * X % p, Y * Y % p
+            C = B * B % p
+            D = 2 * ((X + B) ** 2 - A - C) % p
+            E = 3 * A % p
+            X3 = (E * E - 2 * D) % p
+            Y, Z = (E * (D - X3) - 8 * C) % p, 2 * Y * Z % p
+            X = X3
+        if bit == "1":                      # mixed addition of the affine P (madd-2007-bl), with its special cases
+            if not Z:
+                X, Y, Z = x2, y2, 1
+                continue
+            Z2 = Z * Z % p
+            U2, S2 = x2 * Z2 % p, y2 * Z * Z2 % p
+            H, rr = (U2 - X) % p, (S2 - Y) % p
+            if H == 0:
+                if rr:
+                    X, Y, Z = 1, 1, 0
+                    continue
+                A, B = X * X % p, Y * Y % p          # P + P: double
+                C = B * B % p
+                D = 2 * ((X + B) ** 2 - A - C) % p
+                E = 3 * A % p
+                X3 = (E * E - 2 * D) % p
+                Y, Z = (E * (D - X3) - 8 * C) % p, 2 * Y * Z % p
+                X = X3
+                continue
+            HH = H * H % p
+            HHH = H * HH % p
+            V = X * HH % p
+            X3 = (rr * rr - HHH - 2 * V) % p
+            Y, Z = (rr * (V - X3) - Y * HHH) % p, Z * H % p
+            X = X3
+    if not Z:
+        return None
+    zi = pow(Z, -1, p)
+    zi2 = zi * zi % p
+    return X * zi2 % p, Y * zi2 * zi % p
 
 
 def msm_naive(curve_id, bases, scalars):
