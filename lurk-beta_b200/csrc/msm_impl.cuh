@@ -17,10 +17,11 @@
 //      independent of the bucket sizes (perfect balance for any scalar distribution).  A thread gathers its bases
 //      with 128-bit loads (next point prefetched during the current addition), adds them in XYZZ coordinates
 //      (8M+2S mixed addition, no inversions) and flushes a bucket sum whenever the bucket id changes.  The first run
-//      of a segment may continue a bucket started by the previous thread: it goes to a (key, point) partial list
-//      which is reduced by the same rule in a few geometrically shrinking passes.
-//   5. per-window running-sum reduction (chunks of buckets in parallel, then one CTA per window).
-//   6. host: Horner combine of the <= 64 window sums and one inversion to affine.
+//      of a segment may continue a bucket started by the previous thread: it is stored as that thread's partial sum.
+//   5. merge: bucket b adds the partials of the threads whose segment starts strictly inside it -- a contiguous range of
+//      thread indices found from the offsets alone (one thread per bucket; one CTA per listed long bucket).
+//   6. per-window running-sum reduction (chunks of buckets in parallel, then one CTA per window).
+//   7. host: Horner combine of the <= 64 window sums and one inversion to affine.
 // Integer-ALU bound: ~10 Montgomery products per (scalar, window); algorithmic traffic 96 B per term.
 #pragma once
 #include "common.cuh"
@@ -165,15 +166,38 @@ static __global__ void __launch_bounds__(1024) msm_scan_tiles_kernel(const uint3
     for (int k = 0; k < 4; k++) { if (base + k < ntiles) tile_offsets[base + k] = run; run += v[k]; }
     if (threadIdx.x == 0) tile_offsets[ntiles] = total;
 }
+// Level-1 threads of the bucket accumulation whose segment [t * seg, ..) starts strictly inside bucket [lo, hi): each leaves
+// one partial sum of the bucket, ppt[first .. first + count).  The thread holding `lo` writes the bucket itself.
+struct BucketPartials { uint32_t first, count; };
+__host__ __device__ __forceinline__ BucketPartials bucket_partials(uint32_t lo, uint32_t hi, uint32_t seg) {
+    BucketPartials r{lo / seg + 1, 0};
+    if (hi >= lo + 2) {
+        const uint32_t last = (hi - 1) / seg;
+        if (last >= r.first) r.count = last - r.first + 1;
+    }
+    return r;
+}
+// buckets with more partials than this are merged by a whole CTA (msm_merge_long_kernel); the others by one thread each
+static constexpr uint32_t MSM_LONG_PARTIALS = 16;
+
+// long_list (optional): appends every bucket with more than MSM_LONG_PARTIALS partials for segments of `seg` entries;
+// long_list[-1] is its length, zeroed before the launch
 static __global__ void __launch_bounds__(1024) msm_scan_apply_kernel(const uint32_t *__restrict__ counts, uint32_t len, const uint32_t *__restrict__ tile_offsets,
-                                                              uint32_t ntiles, uint32_t *__restrict__ offsets) {
+                                                              uint32_t ntiles, uint32_t *__restrict__ offsets, uint32_t seg = 0,
+                                                              uint32_t *long_list = nullptr) {
     const uint32_t base = blockIdx.x * SCAN_TILE + threadIdx.x * 4;
     uint32_t v[4], sum = 0;
 #pragma unroll
     for (int k = 0; k < 4; k++) { v[k] = base + k < len ? counts[base + k] : 0; sum += v[k]; }
     uint32_t run = tile_offsets[blockIdx.x] + block_exclusive_scan_1024(sum, nullptr);
 #pragma unroll
-    for (int k = 0; k < 4; k++) { if (base + k < len) offsets[base + k] = run; run += v[k]; }
+    for (int k = 0; k < 4; k++) {
+        if (base + k < len) {
+            offsets[base + k] = run;
+            if (long_list && bucket_partials(run, run + v[k], seg).count > MSM_LONG_PARTIALS) long_list[atomicAdd(long_list - 1, 1u)] = base + k;
+        }
+        run += v[k];
+    }
     if (blockIdx.x == 0 && threadIdx.x == 0) offsets[len] = tile_offsets[ntiles];
 }
 
@@ -235,13 +259,13 @@ __device__ __forceinline__ void store_xyzz(XYZZ<Fb> *p, const XYZZ<Fb> &a) {
 template <class Fb, int MINB, bool DIRECT = false>
 __global__ void __launch_bounds__(128, MINB) msm_accumulate_kernel(const uint32_t *__restrict__ offsets, uint32_t nbuckets,
                                                              const uint32_t *__restrict__ sorted, const Affine<Fb> *__restrict__ bases,
-                                                             XYZZ<Fb> *__restrict__ bucket_acc, uint32_t *__restrict__ pkey,
-                                                             XYZZ<Fb> *__restrict__ ppt, uint32_t seg, uint32_t nthreads) {
+                                                             XYZZ<Fb> *__restrict__ bucket_acc, XYZZ<Fb> *__restrict__ ppt, uint32_t seg,
+                                                             uint32_t nthreads) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= nthreads) return;
     const uint32_t total = offsets[nbuckets];
     const uint64_t start64 = (uint64_t)t * seg;
-    if (start64 >= total) { pkey[t] = KEY_NONE; return; }
+    if (start64 >= total) return;
     const uint32_t start = (uint32_t)start64;
     const uint32_t end = (uint32_t)min((uint64_t)total, start64 + seg);
     // bucket containing `start`: largest key with offsets[key] <= start
@@ -252,7 +276,9 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate_kernel(const uint32_
     }
     uint32_t key = lo;
     uint32_t run_end = min(offsets[key + 1], end);
-    bool first_run = true;
+    // a first run that starts inside its bucket continues another thread's run: it becomes the partial ppt[t], which
+    // msm_merge_kernel adds to the bucket (see bucket_partials); every other run starts its bucket and writes it
+    bool first_run = offsets[key] != start;
     uint32_t e_next = DIRECT ? start : sorted[start];
     Affine<Fb> p_next = load_affine(bases + (e_next & 0x7fffffffu));
     XYZZ<Fb> acc = XYZZ<Fb>::identity();
@@ -269,7 +295,7 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate_kernel(const uint32_
         }
         acc.add_affine(p, (e >> 31) != 0);
         if (pos == run_end) {
-            if (first_run) { pkey[t] = key; store_xyzz(ppt + t, acc); first_run = false; }
+            if (first_run) { store_xyzz(ppt + t, acc); first_run = false; }
             else store_xyzz(bucket_acc + key, acc);   // this run starts exactly at the bucket start: sole initialiser
             acc = XYZZ<Fb>::identity();
             if (pos < end) {
@@ -416,73 +442,49 @@ __global__ void __launch_bounds__(128) msm_pair_kernel(const uint32_t *__restric
     }
 }
 
-// levels >= 2: the same rule on (key, point) lists; keys are non-decreasing, KEY_NONE only as a tail
+// ---- merge of the level-1 partials: bucket b receives the partials ppt[first .. first + count) of the threads whose segment
+// starts strictly inside it (bucket_partials), a contiguous range, so no keys and no search are needed.  Every bucket is
+// written here or by the long-bucket kernel (empty buckets as the identity), so bucket_acc is not cleared before a launch.
+// Longest chain: MSM_LONG_PARTIALS additions here, ceil(partials / 256) + 8 in msm_merge_long_kernel -- instead of the
+// 8 + 5 per pass of the shrinking (key, point) passes this replaces, which also walked one slot per level-1 thread.
+static constexpr uint32_t MSM_MERGE_THREADS = 64, MSM_MERGE_LONG_THREADS = 256;
 template <class Fb>
-__global__ void __launch_bounds__(128) msm_partial_kernel(const uint32_t *__restrict__ keys_in, const XYZZ<Fb> *__restrict__ pts_in,
-                                                          uint32_t count, XYZZ<Fb> *__restrict__ bucket_acc, uint32_t *__restrict__ keys_out,
-                                                          XYZZ<Fb> *__restrict__ pts_out, uint32_t seg, int last_level) {
-    const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
-    const uint64_t s64 = (uint64_t)u * seg;
-    if (s64 >= count) return;
-    const uint32_t s = (uint32_t)s64, e = (uint32_t)min((uint64_t)count, s64 + seg);
-    uint32_t cur = KEY_NONE;
-    bool first_run = true, wrote_out = false;
+__global__ void __launch_bounds__(MSM_MERGE_THREADS) msm_merge_kernel(const uint32_t *__restrict__ offsets, uint32_t nbuckets, uint32_t seg,
+                                                                      const XYZZ<Fb> *__restrict__ ppt, XYZZ<Fb> *__restrict__ bucket_acc) {
+    const uint32_t b = blockIdx.x * MSM_MERGE_THREADS + threadIdx.x;
+    if (b >= nbuckets) return;
+    const uint32_t lo = offsets[b], hi = offsets[b + 1];
+    const BucketPartials bp = bucket_partials(lo, hi, seg);
+    if (bp.count > MSM_LONG_PARTIALS) return;                    // msm_merge_long_kernel's
     XYZZ<Fb> acc = XYZZ<Fb>::identity();
-    for (uint32_t i = s; i <= e; i++) {
-        const uint32_t k = i < e ? keys_in[i] : KEY_NONE;   // one extra step flushes the last run
-        if (k == cur && k != KEY_NONE) { acc.add(load_xyzz(pts_in + i)); continue; }
-        if (cur != KEY_NONE) {
-            if (first_run && !last_level) { keys_out[u] = cur; store_xyzz(pts_out + u, acc); wrote_out = true; }
-            else { XYZZ<Fb> b = load_xyzz(bucket_acc + cur); b.add(acc); store_xyzz(bucket_acc + cur, b); }
-            first_run = false;
+    if (hi > lo) acc = load_xyzz(bucket_acc + b);
+    for (uint32_t i = 0; i < bp.count; i++) acc.add(load_xyzz(ppt + bp.first + i));
+    store_xyzz(bucket_acc + b, acc);
+}
+
+// the long buckets listed by msm_scan_apply_kernel (0/1-heavy witness vectors, equal scalars, the shared bucket set of
+// fixed-base mode): one bucket per CTA at a time, strided sums, then a shared-memory tree
+template <class Fb>
+__global__ void __launch_bounds__(MSM_MERGE_LONG_THREADS) msm_merge_long_kernel(const uint32_t *__restrict__ offsets, uint32_t seg,
+                                                                                const XYZZ<Fb> *__restrict__ ppt, const uint32_t *__restrict__ long_list,
+                                                                                XYZZ<Fb> *__restrict__ bucket_acc) {
+    __shared__ XYZZ<Fb> sm[MSM_MERGE_LONG_THREADS];
+    const uint32_t tid = threadIdx.x, nlong = long_list[-1];
+    for (uint32_t i = blockIdx.x; i < nlong; i += gridDim.x) {
+        const uint32_t b = long_list[i];
+        const BucketPartials bp = bucket_partials(offsets[b], offsets[b + 1], seg);
+        XYZZ<Fb> acc = XYZZ<Fb>::identity();
+        if (tid == 0) acc = load_xyzz(bucket_acc + b);            // a long bucket is not empty
+        for (uint32_t j = tid; j < bp.count; j += MSM_MERGE_LONG_THREADS) acc.add(load_xyzz(ppt + bp.first + j));
+        sm[tid] = acc;
+        __syncthreads();
+        for (uint32_t stride = MSM_MERGE_LONG_THREADS / 2; stride > 0; stride >>= 1) {
+            if (tid < stride) { XYZZ<Fb> x = sm[tid]; x.add(sm[tid + stride]); sm[tid] = x; }
+            __syncthreads();
         }
-        if (k == KEY_NONE) break;
-        cur = k;
-        acc = load_xyzz(pts_in + i);
+        if (tid == 0) store_xyzz(bucket_acc + b, sm[0]);
+        __syncthreads();                                          // sm is reused by the next long bucket
     }
-    if (!wrote_out && !last_level) keys_out[u] = KEY_NONE;
-}
-
-template <class Fb>
-__device__ __forceinline__ XYZZ<Fb> shfl_up_xyzz(const XYZZ<Fb> &p, int d) {
-    XYZZ<Fb> r;
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-        r.x.v[i] = __shfl_up_sync(0xffffffffu, p.x.v[i], d);
-        r.y.v[i] = __shfl_up_sync(0xffffffffu, p.y.v[i], d);
-        r.zz.v[i] = __shfl_up_sync(0xffffffffu, p.zz.v[i], d);
-        r.zzz.v[i] = __shfl_up_sync(0xffffffffu, p.zzz.v[i], d);
-    }
-    return r;
-}
-
-// Later levels are latency-bound (few entries): one warp takes 32 consecutive (key, point) entries and combines equal
-// keys with a segmented Hillis-Steele scan over shuffles -- 5 dependent additions per 32x shrink instead of 32.
-template <class Fb>
-__global__ void __launch_bounds__(128) msm_partial_warp_kernel(const uint32_t *__restrict__ keys_in, const XYZZ<Fb> *__restrict__ pts_in,
-                                                               uint32_t count, XYZZ<Fb> *__restrict__ bucket_acc, uint32_t *__restrict__ keys_out,
-                                                               XYZZ<Fb> *__restrict__ pts_out, int last_level) {
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if ((uint64_t)gw * 32 >= count) return;   // whole warp out of range
-    const uint32_t i = gw * 32 + lane;
-    const uint32_t key = i < count ? keys_in[i] : KEY_NONE;
-    XYZZ<Fb> pt = XYZZ<Fb>::identity();
-    if (key != KEY_NONE) pt = load_xyzz(pts_in + i);
-#pragma unroll 1
-    for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t k2 = __shfl_up_sync(0xffffffffu, key, d);
-        const XYZZ<Fb> p2 = shfl_up_xyzz(pt, d);
-        if (lane >= (uint32_t)d && k2 == key && key != KEY_NONE) pt.add(p2);
-    }
-    const uint32_t first_key = __shfl_sync(0xffffffffu, key, 0);
-    const uint32_t next_key = __shfl_down_sync(0xffffffffu, key, 1);
-    const bool run_end = key != KEY_NONE && (lane == 31 || next_key != key);
-    if (run_end) {
-        if (key == first_key && !last_level) { keys_out[gw] = key; store_xyzz(pts_out + gw, pt); }
-        else { XYZZ<Fb> b = load_xyzz(bucket_acc + key); b.add(pt); store_xyzz(bucket_acc + key, b); }
-    }
-    if (first_key == KEY_NONE && lane == 0 && !last_level) keys_out[gw] = KEY_NONE;
 }
 
 // ---- bucket reduction: R_w = sum_b (b + 1) B_{w,b} per window, in three short, wide kernels.
@@ -660,7 +662,7 @@ __global__ void __launch_bounds__(256) msm_bases_to_mont_kernel(Fb *coords, size
 
 // ----------------------------------------------------------------------------- context
 struct MsmScratch {
-    DevBuf counts, offsets, tiles, sorted, buckets, pkey[2], ppt[2], chunks, chunk_sums, slices, wins, result, scalars, pair_offs[2], pair_pts[2];
+    DevBuf counts, offsets, tiles, sorted, buckets, ppt, chunks, chunk_sums, slices, wins, result, scalars, pair_offs[2], pair_pts[2];
     void *h_wins = nullptr;   // pinned
     void *h_stage[2] = {nullptr, nullptr};          // pinned staging for host-buffer scalars
     cudaEvent_t stage_done[2] = {nullptr, nullptr};
@@ -776,19 +778,17 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     for (int r = 0; r < rounds; r++) cap_final = cap_final / 2 + TB + 1;       // sum of ceil(m_k / 2) <= cap / 2 + buckets
     const uint32_t t1 = rounds ? (uint32_t)((cap_final + P.seg - 1) / P.seg) : P.t1;
     const uint32_t t1_alloc = std::max(t1, P.t1);
+    // a long bucket holds more than MSM_LONG_PARTIALS segment starts, so there are at most t1 / (MSM_LONG_PARTIALS + 1)
+    const uint32_t max_long = t1 / (MSM_LONG_PARTIALS + 1) + 1;
     {
         // scratch grows monotonically; a context is normally run at one size (the circuit's witness length)
         auto ensure = [](DevBuf &b, size_t bytes) { return b.bytes >= bytes ? LURK_OK : b.alloc(bytes); };
-        LURK_TRY(ensure(S.counts, ((size_t)TB + 1) * 2 * sizeof(uint32_t)));   // counts | cursor
+        LURK_TRY(ensure(S.counts, (((size_t)TB + 1) * 2 + 1 + max_long) * sizeof(uint32_t)));   // counts | cursor | long count | long list
         LURK_TRY(ensure(S.offsets, ((size_t)TB + 1) * sizeof(uint32_t)));
         LURK_TRY(ensure(S.tiles, ((size_t)ntiles + 1) * 2 * sizeof(uint32_t)));  // tile sums | tile offsets
         LURK_TRY(ensure(S.sorted, n * (size_t)P.nwin * sizeof(uint32_t)));
         LURK_TRY(ensure(S.buckets, (size_t)TB * sizeof(Pt)));
-        LURK_TRY(ensure(S.pkey[0], (size_t)t1_alloc * sizeof(uint32_t)));
-        LURK_TRY(ensure(S.ppt[0], (size_t)t1_alloc * sizeof(Pt)));
-        size_t t2 = ((size_t)t1_alloc + 7) / 8;
-        LURK_TRY(ensure(S.pkey[1], t2 * sizeof(uint32_t)));
-        LURK_TRY(ensure(S.ppt[1], t2 * sizeof(Pt)));
+        LURK_TRY(ensure(S.ppt, (size_t)t1_alloc * sizeof(Pt)));              // one partial slot per level-1 thread
         const size_t nchunks_all = (size_t)P.rwin * P.G;
         LURK_TRY(ensure(S.chunks, nchunks_all * sizeof(Pt)));          // tri_g
         LURK_TRY(ensure(S.chunk_sums, nchunks_all * sizeof(Pt)));      // run_g
@@ -802,10 +802,10 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     uint32_t *offsets = S.offsets.as<uint32_t>();
     uint32_t *tile_sums = S.tiles.as<uint32_t>(), *tile_offsets = tile_sums + (ntiles + 1);
     uint32_t *sorted = S.sorted.as<uint32_t>();
-    Pt *buckets = S.buckets.as<Pt>();
+    uint32_t *long_list = cursor + (TB + 1) + 1;                        // long_list[-1] is zeroed with the counts
+    Pt *buckets = S.buckets.as<Pt>();       // every bucket is written by the accumulation or the merge: no clearing
 
-    LURK_CUDA_TRY(cudaMemsetAsync(counts, 0, ((size_t)TB + 1) * 2 * sizeof(uint32_t), s));
-    LURK_CUDA_TRY(cudaMemsetAsync(buckets, 0, (size_t)TB * sizeof(Pt), s));   // all-zero = identity
+    LURK_CUDA_TRY(cudaMemsetAsync(counts, 0, (((size_t)TB + 1) * 2 + 1) * sizeof(uint32_t), s));
     const unsigned gs = (unsigned)((n + 255) / 256);
     unsigned launches = 0;
     const uint32_t key_stride = fixed ? 0u : P.nb;                 // fixed-base: all windows share one bucket set
@@ -815,7 +815,8 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     msm_count_kernel<Fs><<<gs, 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, counts);
     msm_scan_tile_sums_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_sums);
     msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
-    msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets);
+    // the offsets the accumulation walks also give the merge its long buckets (after the last pair round, if any)
+    msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, rounds ? nullptr : long_list);
     msm_scatter_kernel<Fs><<<gs, 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, base_stride, offsets, cursor, sorted);
     if (ctx->profile) LURK_CUDA_TRY(cudaEventRecord(ctx->ev0, s));
     // ---- pair rounds
@@ -831,7 +832,7 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
         msm_halve_kernel<<<(TB + 256) / 256, 256, 0, s>>>(acc_offs, TB, counts);          // `counts` is free after the scatter
         msm_scan_tile_sums_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_sums);
         msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
-        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, o2);
+        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, o2, P.seg, r == rounds - 1 ? long_list : nullptr);
         const size_t pthreads = (cap_r + PAIR_B - 1) / PAIR_B;
         const unsigned pgrid = (unsigned)((pthreads + 127) / 128);
         if (r == 0) msm_pair_kernel<Fb, true><<<pgrid, 128, 0, s>>>(acc_offs, o2, TB, sorted, acc_pts, pb.as<Affine<Fb>>());
@@ -841,38 +842,19 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
         acc_pts = pb.as<Affine<Fb>>();
     }
     if (rounds)
-        msm_accumulate_kernel<Fb, 5, true><<<(t1 + 127) / 128, 128, 0, s>>>(acc_offs, TB, sorted, acc_pts, buckets, S.pkey[0].as<uint32_t>(),
-                                                                              S.ppt[0].as<Pt>(), P.seg, t1);
+        msm_accumulate_kernel<Fb, 5, true><<<(t1 + 127) / 128, 128, 0, s>>>(acc_offs, TB, sorted, acc_pts, buckets, S.ppt.as<Pt>(), P.seg, t1);
     else if (fixed)
-        msm_accumulate_kernel<Fb, 5><<<(P.t1 + 127) / 128, 128, 0, s>>>(offsets, TB, sorted, bases, buckets, S.pkey[0].as<uint32_t>(),
-                                                                         S.ppt[0].as<Pt>(), P.seg, P.t1);
+        msm_accumulate_kernel<Fb, 5><<<(P.t1 + 127) / 128, 128, 0, s>>>(offsets, TB, sorted, bases, buckets, S.ppt.as<Pt>(), P.seg, P.t1);
     else
-        msm_accumulate_kernel<Fb, 4><<<(P.t1 + 127) / 128, 128, 0, s>>>(offsets, TB, sorted, bases, buckets, S.pkey[0].as<uint32_t>(),
-                                                                         S.ppt[0].as<Pt>(), P.seg, P.t1);
+        msm_accumulate_kernel<Fb, 4><<<(P.t1 + 127) / 128, 128, 0, s>>>(offsets, TB, sorted, bases, buckets, S.ppt.as<Pt>(), P.seg, P.t1);
     if (ctx->profile) LURK_CUDA_TRY(cudaEventRecord(ctx->ev1, s));
     launches += 6;
-    // shrinking passes over the partial list: one throughput-shaped pass (8 entries per thread), then warp-cooperative
-    // passes (32x per pass, 5 dependent additions each) until a single warp finishes
-    uint32_t count = t1;
-    int cur = 0;
-    if (count > 32) {
-        const uint32_t seg2 = 8, threads = (count + seg2 - 1) / seg2;
-        msm_partial_kernel<Fb><<<(threads + 127) / 128, 128, 0, s>>>(S.pkey[cur].as<uint32_t>(), S.ppt[cur].as<Pt>(), count, buckets,
-                                                                    S.pkey[cur ^ 1].as<uint32_t>(), S.ppt[cur ^ 1].as<Pt>(), seg2, 0);
-        launches++;
-        count = threads;
-        cur ^= 1;
-    }
-    for (;;) {
-        const uint32_t warps = (count + 31) / 32;
-        const int last = warps == 1;
-        msm_partial_warp_kernel<Fb><<<(warps * 32 + 127) / 128, 128, 0, s>>>(S.pkey[cur].as<uint32_t>(), S.ppt[cur].as<Pt>(), count, buckets,
-                                                                            S.pkey[cur ^ 1].as<uint32_t>(), S.ppt[cur ^ 1].as<Pt>(), last);
-        launches++;
-        if (last) break;
-        count = warps;
-        cur ^= 1;
-    }
+    // merge of the partials into their buckets: long buckets (one CTA each, a grid of at most two per SM walking the list)
+    // and the others (one thread each) are disjoint, so the two launches do not depend on each other
+    msm_merge_long_kernel<Fb><<<std::min<uint32_t>(max_long, 2 * sm_count()), MSM_MERGE_LONG_THREADS, 0, s>>>(acc_offs, P.seg, S.ppt.as<Pt>(),
+                                                                                                             long_list, buckets);
+    msm_merge_kernel<Fb><<<(TB + MSM_MERGE_THREADS - 1) / MSM_MERGE_THREADS, MSM_MERGE_THREADS, 0, s>>>(acc_offs, TB, P.seg, S.ppt.as<Pt>(), buckets);
+    launches += 2;
     // bucket reduction: chunk sums, per-bit tree sums, (slice sums); the host finishes with a Horner over nq points per set
     const uint32_t nchunks = P.rwin * P.G, nres = P.rwin * P.nq;
     if (nres > MSM_MAX_RESULT_POINTS) { set_error("internal: %u result points", nres); return LURK_ERR_ARG; }
