@@ -217,8 +217,8 @@ int lurk_shake256(const uint8_t *in, size_t in_len, uint8_t *out, size_t out_len
  *     spartan::snark::RelaxedR1CSSNARK::prove): sum-check prover rounds over device-resident multilinear polynomials
  *     (SumcheckProof::prove_quad / prove_cubic_with_additive_term: compute_eval_points_* + bind_poly_var_top) and the folding rounds
  *     of the inner-product argument (provider::ipa_pc::InnerProductArgument::prove), the HyperKZG opening prover
- *     (provider::hyperkzg::EvaluationEngine::prove), plus EqPolynomial::evals and the inner product behind
- *     MultilinearPolynomial::evaluate.  The Fiat-Shamir transcript (Keccak256Transcript) stays on the caller's side:
+ *     (provider::hyperkzg::EvaluationEngine::prove), batch_eval_reduce (every evaluation claim of a proof reduced to one opening), plus
+ *     EqPolynomial::evals and the inner product behind MultilinearPolynomial::evaluate.  The Fiat-Shamir transcript (Keccak256Transcript) stays on the caller's side:
  *     every round passes its message to `challenge` and receives the verifier's challenge.  Polynomials: 2^num_rounds elements,
  *     Montgomery form, index bit (num_rounds - 1) = the first variable (bound first), as in Arecibo's MultilinearPolynomial.
  *     Not here: the transcript, proof (de)serialisation, the verifiers (HyperKZG's pairing check) -- CPU / third-party protocol code.
@@ -270,6 +270,21 @@ int lurk_ipa_prove_dev(int curve_id, lurk_msm_ctx *ck, const uint8_t ck_c[64], v
 int lurk_hyperkzg_prove_dev(int curve_id, lurk_msm_ctx *ck, const void *d_poly, const uint8_t *point, int num_vars,
                             lurk_challenge_fn challenge, void *user, uint8_t *com_out, uint8_t *w_out, uint8_t *v_out, int fmt,
                             void *stream);
+/* Arecibo's batch_eval_reduce (with PolyEvalInstance / PolyEvalWitness::batch_diff_size; public crate, not under the reference checkout):
+ * reduces n_claims (1..60) evaluation claims P_i(x_i) = e_i to ONE claim about one polynomial, so that `compress` ends in a single
+ * opening.  d_polys[i]: 2^num_vars[i] Montgomery elements (0 <= num_vars[i] <= 40; NOT modified); points: the x_i concatenated, num_vars[i]
+ * elements each, x_i[0] <-> the top index bit (may be NULL when every num_vars[i] is 0); evals: the e_i.  m = max num_vars[i].
+ *   round 0:      message e_0 | .. | e_{n-1}                 -> rho
+ *   rounds 1..m:  SumcheckProof::prove_quad_batch over (P_i, eq(x_i)), claims e_i, coefficients rho^i, instance i joining late as in
+ *                 lurk_sumcheck_prove_batch_dev; message s(0) | s(1) | s(2)  -> r_{j-1}
+ *   round m + 1:  message L_0 | .. | L_{n-1}, L_i = P_i(r[m - n_i:])   -> gamma
+ * Outputs (any but d_joint may be NULL): round_evals m x 3 x 32; r_out m x 32; claims_left the L_i; weights w_i = gamma^i (the caller
+ * forms the joint commitment sum_i w_i C_i); joint_eval = sum_i gamma^i prod_{j < m - n_i} (1 - r_j) L_i; d_joint (caller-allocated,
+ * 2^m Montgomery elements, not overlapping any P_i) d_joint[k] = sum_{i : k < 2^n_i} gamma^i P_i[k] -- the polynomial to open at r. */
+int lurk_batch_eval_reduce_dev(int field_id, int n_claims, const void *const *d_polys, const int *num_vars,
+                               const uint8_t *points, const uint8_t *evals, lurk_challenge_fn challenge, void *user,
+                               uint8_t *round_evals, uint8_t *r_out, uint8_t *claims_left, uint8_t *weights,
+                               uint8_t joint_eval[32], void *d_joint, int fmt, void *stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * S5  Fold helpers on device-resident vectors (Arecibo NIFS::prove / R1CSShape::commit_T /

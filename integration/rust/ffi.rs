@@ -93,6 +93,10 @@ extern "C" {
                               user: *mut c_void, l_out: *mut u8, r_out: *mut u8, a_final: *mut u8, b_final: *mut u8, fmt: c_int, stream: *mut c_void) -> c_int;
     pub fn lurk_hyperkzg_prove_dev(curve_id: c_int, ck: *mut lurk_msm_ctx, d_poly: *const c_void, point: *const u8, num_vars: c_int, challenge: lurk_challenge_fn,
                                    user: *mut c_void, com_out: *mut u8, w_out: *mut u8, v_out: *mut u8, fmt: c_int, stream: *mut c_void) -> c_int;
+    pub fn lurk_batch_eval_reduce_dev(field_id: c_int, n_claims: c_int, d_polys: *const *const c_void, num_vars: *const c_int, points: *const u8,
+                                      evals: *const u8, challenge: lurk_challenge_fn, user: *mut c_void, round_evals: *mut u8, r_out: *mut u8,
+                                      claims_left: *mut u8, weights: *mut u8, joint_eval: *mut u8, d_joint: *mut c_void, fmt: c_int,
+                                      stream: *mut c_void) -> c_int;
 }
 /// `int (*)(void *user, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32])`: the Fiat-Shamir transcript stays in
 /// Rust.  A closure is passed as `user` and trampolined, e.g. for SumcheckProof::prove_*:

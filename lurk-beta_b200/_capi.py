@@ -101,6 +101,7 @@ PROTOTYPES = {
     "lurk_msm_ctx_info": (_i, [_vp, C.POINTER(_i), C.POINTER(_sz)]),
     "lurk_ck_powers_dev": (_i, [_i, _vp, _vp, _sz, _vp, _i, _vp]),
     "lurk_hyperkzg_prove_dev": (_i, [_i, _vp, _vp, _vp, _i, CHALLENGE_FN, _vp, _vp, _vp, _vp, _i, _vp]),
+    "lurk_batch_eval_reduce_dev": (_i, [_i, _i, C.POINTER(_vp), C.POINTER(_i), _vp, _vp, CHALLENGE_FN, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "lurk_axpy_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lurk_spmv_csr_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
     "lurk_cross_term_dev": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),

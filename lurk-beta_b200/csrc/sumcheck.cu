@@ -11,6 +11,8 @@
 //                                Bytes per index pair: K x (4 x 32 read + 2 x 32 written); products: K x 2 + 2 (quad: 4) / 6 (cubic).
 //   eq_kernel                    EqPolynomial::evals: 16 outputs per thread (prefix product over the high bits, doubling over the low 4).
 //   dot_kernel (sc_scratch.cuh)  inner product (MultilinearPolynomial::evaluate = <Z, eq(r)>, IPA's c_L / c_R).
+//   poly_combine_kernel          batch_eval_reduce's joint polynomial sum_i gamma^i P_i in one pass (one read per input, one write per
+//                                output) instead of n - 1 AXPY passes over the output.
 // The inner-product argument lives in ipa.cu.
 // Reductions: per-thread modular sums -> warp shuffles -> shared memory -> one partial per CTA -> the last CTA to finish adds the
 // partials (single launch, no second kernel, no atomics on field elements).
@@ -201,16 +203,8 @@ static int sumcheck_prove_batch(int n_inst, void *const *d_polys, const int *nr,
 }
 
 template <class F>
-static int eq_evals(const uint8_t *tau, int l, void *d_out, int fmt, cudaStream_t s) {
-    EqArgs<F> a;
-    memset(&a, 0, sizeof a);
-    a.l = l;
-    for (int j = 0; j < l; j++) {
-        if (!fe_in(tau + 32 * j, fmt, a.tau[j])) { set_error("tau[%d] is not reduced", j); return LURK_ERR_RANGE; }
-        a.one_minus[j] = F::one() - a.tau[j];
-    }
-    const int to_canonical = fmt == LURK_FMT_CANONICAL;
-    F *out = static_cast<F *>(d_out);
+static int eq_launch(const EqArgs<F> &a, F *out, int to_canonical, cudaStream_t s) {
+    const int l = a.l;
     switch (std::min(l, 4)) {
         case 0: eq_kernel<F, 0><<<1, 128, 0, s>>>(a, out, to_canonical); break;
         case 1: eq_kernel<F, 1><<<1, 128, 0, s>>>(a, out, to_canonical); break;
@@ -219,6 +213,147 @@ static int eq_evals(const uint8_t *tau, int l, void *d_out, int fmt, cudaStream_
         default: eq_kernel<F, 4><<<sc_grid((size_t)1 << (l - 4), 128), 128, 0, s>>>(a, out, to_canonical); break;
     }
     LURK_CUDA_TRY(cudaGetLastError());
+    return LURK_OK;
+}
+
+template <class F>
+static int eq_evals(const uint8_t *tau, int l, void *d_out, int fmt, cudaStream_t s) {
+    EqArgs<F> a;
+    memset(&a, 0, sizeof a);
+    a.l = l;
+    for (int j = 0; j < l; j++) {
+        if (!fe_in(tau + 32 * j, fmt, a.tau[j])) { set_error("tau[%d] is not reduced", j); return LURK_ERR_RANGE; }
+        a.one_minus[j] = F::one() - a.tau[j];
+    }
+    return eq_launch<F>(a, static_cast<F *>(d_out), fmt == LURK_FMT_CANONICAL, s);
+}
+
+// ------------------------------------------------------------------------------------------------ batch_eval_reduce
+// The joint polynomial of the reduction in one pass: out[k] = sum_{t : k < len_t} w_t P_t[k] for k < out_len.  The terms are sorted by
+// length, longest first, so a thread stops at the first one that no longer reaches its index; every output is written once and every
+// input element read once: 32 (sum_t len_t + out_len) bytes, one product per term -- HBM-bound.  The table rides in the kernel
+// parameters (60 x 48 bytes), read as uniform constant-bank loads.
+template <class F>
+struct CombineArgs {
+    struct Term { const F *poly; size_t len; F w; } term[SC_MAX_INSTANCES];
+    int n;
+    size_t out_len;
+};
+
+template <class F>
+__global__ void __launch_bounds__(256) poly_combine_kernel(const __grid_constant__ CombineArgs<F> a, F *__restrict__ out) {
+    for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < a.out_len; k += (size_t)gridDim.x * blockDim.x) {
+        F acc = F::zero();
+        for (int t = 0; t < a.n && k < a.term[t].len; t++) acc += a.term[t].w * load_fe<F>(a.term[t].poly + k);
+        store_fe(out + k, acc);
+    }
+}
+
+// the sum-check's rounds 0 .. m-1 are rounds 1 .. m of the reduction's transcript
+struct ShiftedChallenge { lurk_challenge_fn fn; void *user; };
+static int shifted_challenge(void *user, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32]) {
+    const ShiftedChallenge *c = static_cast<const ShiftedChallenge *>(user);
+    return c->fn(c->user, round + 1, message, message_len, challenge_out);
+}
+
+// stream-ordered scratch, freed (in stream order) when the call returns
+struct StreamBuf {
+    void *p = nullptr;
+    cudaStream_t s = nullptr;
+    ~StreamBuf() { if (p) cudaFreeAsync(p, s); }
+    int alloc(size_t bytes, cudaStream_t st) { s = st; LURK_CUDA_TRY(cudaMallocAsync(&p, bytes ? bytes : 16, st)); return LURK_OK; }
+};
+
+// Arecibo's batch_eval_reduce (spartan/mod.rs in the public crate, not under the reference checkout; restated): claims P_i(x_i) = e_i
+// -> rho; the batched quadratic sum-check of sum_i rho^i sum_y P_i(y) eq(x_i, y), instance i joining in round m - n_i, gives r and the
+// L_i = P_i(r[m - n_i:]); -> gamma.  PolyEvalInstance / PolyEvalWitness::batch_diff_size then treat P_i as zero-padded at the top to
+// 2^m elements, so the joint claim is sum_i gamma^i prod_{j < m - n_i} (1 - r_j) L_i about sum_i gamma^i P_i.
+template <class F>
+static int batch_eval_reduce(int n, const void *const *d_polys, const int *nv, const uint8_t *points, const uint8_t *evals_in,
+                             lurk_challenge_fn challenge, void *user, uint8_t *round_evals, uint8_t *r_out, uint8_t *claims_left,
+                             uint8_t *weights, uint8_t *joint_eval, void *d_joint, int fmt, cudaStream_t s) {
+    int m = 0;
+    size_t total = 0, at = 0;
+    std::vector<EqArgs<F>> eq(n);
+    for (int i = 0; i < n; i++) {
+        F e;
+        if (!fe_in(evals_in + 32 * i, fmt, e)) { set_error("evaluation %d is not reduced", i); return LURK_ERR_RANGE; }
+        if (nv[i] > 32) { set_error("claim %d has %d variables; the eq table takes at most 32", i, nv[i]); return LURK_ERR_ARG; }
+        memset(&eq[i], 0, sizeof(EqArgs<F>));
+        eq[i].l = nv[i];
+        for (int j = 0; j < nv[i]; j++, at++) {
+            if (!fe_in(points + 32 * at, fmt, eq[i].tau[j])) { set_error("point %d, coordinate %d is not reduced", i, j); return LURK_ERR_RANGE; }
+            eq[i].one_minus[j] = F::one() - eq[i].tau[j];
+        }
+        m = std::max(m, nv[i]);
+        total += (size_t)1 << nv[i];
+    }
+    uint8_t cb[32];
+    F rho, gamma;
+    int rc = challenge(user, 0, evals_in, (size_t)n * 32, cb);
+    if (rc != 0) { set_error("challenge callback failed in round 0 (%d)", rc); return LURK_ERR_ARG; }
+    if (!fe_in(cb, fmt, rho)) { set_error("challenge of round 0 is not reduced"); return LURK_ERR_RANGE; }
+
+    // working copies (the sum-check binds in place) and eq(x_i) beside them: [P_0 .. P_{n-1} | eq_0 .. eq_{n-1}]
+    StreamBuf work;
+    LURK_TRY(work.alloc(2 * total * sizeof(F), s));
+    F *base = static_cast<F *>(work.p);
+    std::vector<void *> polys(2 * n);
+    std::vector<uint8_t> coeffs(32 * (size_t)n);
+    F c = F::one();
+    for (size_t i = 0, off = 0; i < (size_t)n; off += (size_t)1 << nv[i], i++) {
+        const size_t len = (size_t)1 << nv[i];
+        polys[2 * i] = base + off;
+        polys[2 * i + 1] = base + total + off;
+        LURK_CUDA_TRY(cudaMemcpyAsync(polys[2 * i], d_polys[i], len * sizeof(F), cudaMemcpyDeviceToDevice, s));
+        LURK_TRY(eq_launch<F>(eq[i], static_cast<F *>(polys[2 * i + 1]), 0, s));
+        fe_out(c, fmt, coeffs.data() + 32 * i);
+        c = c * rho;
+    }
+    std::vector<uint8_t> r_bytes(32 * (size_t)std::max(m, 1)), fin(64 * (size_t)n);
+    ShiftedChallenge shifted{challenge, user};
+    LURK_TRY((sumcheck_prove_batch<F, SC_QUAD>(n, polys.data(), nv, evals_in, coeffs.data(), shifted_challenge, &shifted, round_evals,
+                                               r_bytes.data(), fin.data(), fmt, s)));
+
+    // round m + 1: the L_i -> gamma
+    std::vector<uint8_t> left(32 * (size_t)n);
+    for (int i = 0; i < n; i++) memcpy(left.data() + 32 * i, fin.data() + 64 * i, 32);
+    rc = challenge(user, m + 1, left.data(), left.size(), cb);
+    if (rc != 0) { set_error("challenge callback failed in round %d (%d)", m + 1, rc); return LURK_ERR_ARG; }
+    if (!fe_in(cb, fmt, gamma)) { set_error("challenge of round %d is not reduced", m + 1); return LURK_ERR_RANGE; }
+
+    std::vector<F> r(m);
+    for (int j = 0; j < m; j++) fe_in(r_bytes.data() + 32 * j, fmt, r[j]);
+    CombineArgs<F> args;
+    memset(&args, 0, sizeof args);
+    args.n = n;
+    args.out_len = (size_t)1 << m;
+    std::vector<int> order(n);
+    for (int i = 0; i < n; i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return nv[a] > nv[b]; });
+    std::vector<F> w(n);
+    F joint = F::zero();
+    w[0] = F::one();
+    for (int i = 1; i < n; i++) w[i] = w[i - 1] * gamma;
+    for (int i = 0; i < n; i++) {
+        F L, scale = w[i];
+        fe_in(left.data() + 32 * i, fmt, L);
+        for (int j = 0; j < m - nv[i]; j++) scale = scale * (F::one() - r[j]);
+        joint += scale * L;
+    }
+    for (int t = 0; t < n; t++) {
+        const int i = order[t];
+        args.term[t].poly = static_cast<const F *>(d_polys[i]);
+        args.term[t].len = (size_t)1 << nv[i];
+        args.term[t].w = w[i];
+    }
+    poly_combine_kernel<F><<<sc_grid(args.out_len, 256), 256, 0, s>>>(args, static_cast<F *>(d_joint));
+    LURK_CUDA_TRY(cudaGetLastError());
+    if (r_out) memcpy(r_out, r_bytes.data(), 32 * (size_t)m);
+    if (claims_left) memcpy(claims_left, left.data(), left.size());
+    if (weights)
+        for (int i = 0; i < n; i++) fe_out(w[i], fmt, weights + 32 * i);
+    if (joint_eval) fe_out(joint, fmt, joint_eval);
     return LURK_OK;
 }
 
@@ -255,6 +390,33 @@ int lurk_sumcheck_prove_dev(int field_id, int kind, void *const *d_polys, int nu
                             void *user, uint8_t *round_evals, uint8_t *challenges, uint8_t *final_evals, int fmt, void *stream) {
     return lurk_sumcheck_prove_batch_dev(field_id, kind, 1, d_polys, &num_rounds, claim, nullptr, challenge, user, round_evals, challenges, final_evals,
                                          fmt, stream);
+}
+
+int lurk_batch_eval_reduce_dev(int field_id, int n_claims, const void *const *d_polys, const int *num_vars, const uint8_t *points,
+                               const uint8_t *evals, lurk_challenge_fn challenge, void *user, uint8_t *round_evals, uint8_t *r_out,
+                               uint8_t *claims_left, uint8_t *weights, uint8_t joint_eval[32], void *d_joint, int fmt, void *stream) {
+    if (!d_polys || !num_vars || !evals || !challenge || !d_joint) { set_error("null argument"); return LURK_ERR_ARG; }
+    if (n_claims < 1 || n_claims > SC_MAX_INSTANCES) { set_error("1..%d claims, got %d", SC_MAX_INSTANCES, n_claims); return LURK_ERR_ARG; }
+    if (fmt != LURK_FMT_CANONICAL && fmt != LURK_FMT_MONTGOMERY) { set_error("bad format %d", fmt); return LURK_ERR_ARG; }
+    int m = 0;
+    for (int i = 0; i < n_claims; i++) {
+        if (num_vars[i] < 0 || num_vars[i] > 40) { set_error("bad number of variables %d (claim %d)", num_vars[i], i); return LURK_ERR_ARG; }
+        if (!d_polys[i]) { set_error("polynomial %d is null", i); return LURK_ERR_ARG; }
+        m = std::max(m, num_vars[i]);
+    }
+    if (m > 0 && !points) { set_error("null points"); return LURK_ERR_ARG; }
+    // d_joint is written while the P_i are read: it must not overlap any of them
+    const uintptr_t j0 = reinterpret_cast<uintptr_t>(d_joint), j1 = j0 + ((uintptr_t)32 << m);
+    for (int i = 0; i < n_claims; i++) {
+        const uintptr_t p0 = reinterpret_cast<uintptr_t>(d_polys[i]), p1 = p0 + ((uintptr_t)32 << num_vars[i]);
+        if (p0 < j1 && j0 < p1) { set_error("d_joint overlaps polynomial %d", i); return LURK_ERR_ARG; }
+    }
+    LURK_TRY(require_gpu());
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    return dispatch_field(field_id, [&](auto f) {
+        return batch_eval_reduce<decltype(f)>(n_claims, d_polys, num_vars, points, evals, challenge, user, round_evals, r_out, claims_left, weights,
+                                              joint_eval, d_joint, fmt, s);
+    });
 }
 
 int lurk_eq_evals_dev(int field_id, const uint8_t *tau, int num_vars, void *d_out, int fmt, void *stream) {

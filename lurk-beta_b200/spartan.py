@@ -161,6 +161,38 @@ def hyperkzg_prove(curve_id, ck, d_poly_ptr, point, challenge, stream=0):
     return pts(com, l - 1), [vi[t * l:(t + 1) * l] for t in range(3)], pts(w, 3)
 
 
+def batch_eval_reduce(field_id, claims, challenge, d_joint_ptr=None, stream=0):
+    """Arecibo's batch_eval_reduce: the claims P_i(x_i) = e_i become one claim about sum_i gamma^i P_i (zero-padded to 2^m) at r.
+    claims: [(d_ptr, num_vars, point ints, eval int)], P_i Montgomery on the device (not modified).  challenge(round, message) -> int with
+    round 0 = the evaluations (-> rho), 1..m = the sum-check rounds, m + 1 = the L_i (-> gamma).  d_joint_ptr: 2^m elements of device
+    memory for the joint polynomial (None: allocated here).  Returns (round_evals, r, claims_left, weights, joint_eval, joint tensor or None)."""
+    import torch
+    n = len(claims)
+    nv = [int(c[1]) for c in claims]
+    m = max(nv) if nv else 0
+    joint = None
+    if d_joint_ptr is None:
+        joint = torch.empty((1 << m) * 32, dtype=torch.uint8, device="cuda")
+        d_joint_ptr = joint.data_ptr()
+    ptrs = (C.c_void_p * max(n, 1))(*[C.c_void_p(c[0]) for c in claims])
+    nvs = (C.c_int * max(n, 1))(*nv)
+    pts = np.frombuffer(b"".join(int(x).to_bytes(32, "little") for c in claims for x in c[2]) or bytes(32), dtype=np.uint8).copy()
+    ev = np.frombuffer(b"".join(int(c[3]).to_bytes(32, "little") for c in claims) or bytes(32), dtype=np.uint8).copy()
+    rounds = np.zeros(max(1, m) * 3 * 32, dtype=np.uint8)
+    r = np.zeros(max(1, m) * 32, dtype=np.uint8)
+    left, w, je = np.zeros(max(1, n) * 32, dtype=np.uint8), np.zeros(max(1, n) * 32, dtype=np.uint8), np.zeros(32, dtype=np.uint8)
+    errors = []
+    cb = _callback(challenge, errors)
+    rc = _capi.lib().lurk_batch_eval_reduce_dev(field_id, n, ptrs, nvs, _capi.np_ptr(pts), _capi.np_ptr(ev), cb, None, _capi.np_ptr(rounds),
+                                                _capi.np_ptr(r), _capi.np_ptr(left), _capi.np_ptr(w), _capi.np_ptr(je), C.c_void_p(d_joint_ptr),
+                                                _capi.FMT_CANONICAL, C.c_void_p(stream))
+    if errors:
+        raise errors[0]
+    _capi.check(rc)
+    ri = _ints(rounds)
+    return ([ri[3 * j:3 * j + 3] for j in range(m)], _ints(r)[:m], _ints(left)[:n], _ints(w)[:n], int.from_bytes(je.tobytes(), "little"), joint)
+
+
 
 # ------------------------------------------------------------------------------------------------ RelaxedR1CSSNARK::prove, the GPU half
 class DeviceCSR:
@@ -291,3 +323,119 @@ class RelaxedR1CSProver:
         eval_W = inner_product(f, d_z.data_ptr(), eq_ry.data_ptr(), nv)
         mark("eval W", t0)
         return dict(outer_rounds=outer_rounds, inner_rounds=inner_rounds, claims=claims, eval_W=eval_W, rx=rx, ry=ry, E_padded=E)
+
+
+# ------------------------------------------------------------------------------------------------ BatchedRelaxedR1CSSNARK::prove, the GPU half
+class BatchedRelaxedR1CSProver:
+    """Control flow of Arecibo's spartan::batched::BatchedRelaxedR1CSSNARK::prove -- SuperNova's `compress` over the running instances of
+    every circuit index (reference src/proof/supernova.rs:110,293-317) -- over the C-ABI primitives, every vector device-resident.  Each
+    circuit keeps one RelaxedR1CSProver for its device matrices, transposes and pad_z.  Instance i has 2^s_i rows and 2^(t_i + 1) entries
+    of z; the batched sum-checks let the smaller instances join late.  The challenge labels are those of the test oracle (tests/batched_oracle.py):
+      "tau" (N) -> tau, instance i's table eq(tau, tau^2, tau^4, .., tau^(2^(s_i - 1))) (PowPolynomial::evals_with_powers);
+      "outer_r" (N) -> the outer coefficients outer_r^i;  "outer" (round, s(0..3)) -> r_x;
+      "inner_r" (the claims (Az, Bz, Cz, E)(rx_i) per instance) -> r, coefficients (r^3)^i;  "inner" (round, s(0..2)) -> r_y;
+      "batch_eval" (round, message) -> the challenges of batch_eval_reduce over [W_0 .. W_{N-1}, E_0 .. E_{N-1}].
+    The opening of the joint polynomial (hyperkzg_prove / ipa_prove) is a separate call."""
+
+    def __init__(self, field_id, circuits):
+        """circuits: [(mats, n_w, n_x)] per circuit index, mats as RelaxedR1CSProver takes them"""
+        self.field = field_id
+        self.p = int.from_bytes(field_modulus(field_id), "little")
+        self.provers = [RelaxedR1CSProver(field_id, mats, n_w, n_x) for mats, n_w, n_x in circuits]
+
+    def pad_z(self, i, d_W, u, X):
+        return self.provers[i].pad_z(d_W, u, X)
+
+    def prove(self, instances, challenge, timings=None):
+        """instances: [(d_z, d_E, u)] per circuit (d_z from pad_z, d_E of `rows` Montgomery elements).  Returns the transcript (outer_rounds,
+        inner_rounds, claims, eval_W, reduce_rounds, claims_left), the per-instance points rx / ry, and the reduction's r, weights, joint_eval
+        and joint polynomial (device tensor, 2^m Montgomery elements) together with the padded E vectors."""
+        import time
+        import torch
+        f, p, N = self.field, self.p, len(self.provers)
+        assert len(instances) == N
+        S = [pr.log_rows for pr in self.provers]
+        T = [pr.num_vars.bit_length() for pr in self.provers]            # log2 of the padded z = t_i + 1
+        t = time.perf_counter
+
+        def mark(name, t0):
+            if timings is not None:
+                torch.cuda.synchronize()
+                timings[name] = timings.get(name, 0.0) + (t() - t0) * 1e3
+
+        def cb(label):
+            return lambda rnd, msg: challenge(label, (rnd, _ints(np.frombuffer(msg, dtype=np.uint8)))) % p
+
+        def vec(n):
+            return torch.zeros(n * 32, dtype=torch.uint8, device="cuda")
+
+        t0 = t()
+        tau = challenge("tau", N) % p
+        work, Cz, E = [], [], []
+        for pr, s, (d_z, d_E, u) in zip(self.provers, S, instances):
+            Az, Bz, cz = vec(1 << s), vec(1 << s), vec(1 << s)
+            for M, y in zip(pr.M, (Az, Bz, cz)):
+                M.mv(f, d_z.data_ptr(), y.data_ptr())
+            e = vec(1 << s)
+            e[:pr.rows * 32] = d_E[:pr.rows * 32]
+            uCzE = torch.empty_like(e)
+            pr._axpy(e, cz, u, uCzE)
+            powers = [tau]
+            while len(powers) < s:
+                powers.append(powers[-1] * powers[-1] % p)
+            eq_tau = torch.empty_like(e)
+            eq_evals(f, powers, eq_tau.data_ptr())
+            work.append([eq_tau, Az, Bz, uCzE])
+            Cz.append(cz)
+            E.append(e)
+        mark("multiply_vec + u Cz + E + eq(tau)", t0)
+        t0 = t()
+        outer_r = challenge("outer_r", N) % p
+        outer_rounds, r_x, fin = sumcheck_prove_batch(f, CUBIC, [([w.data_ptr() for w in ws], s) for ws, s in zip(work, S)], [0] * N,
+                                                      [pow(outer_r, i, p) for i in range(N)], cb("outer"))
+        del work
+        mark("outer sum-check (batched)", t0)
+        t0 = t()
+        rx = [r_x[len(r_x) - s:] for s in S]
+        claims, eq_rx = [], []
+        for i, s in enumerate(S):
+            q = vec(1 << s)
+            eq_evals(f, rx[i], q.data_ptr())
+            eq_rx.append(q)
+            claims.append((fin[i][1], fin[i][2], inner_product(f, Cz[i].data_ptr(), q.data_ptr(), 1 << s), inner_product(f, E[i].data_ptr(), q.data_ptr(), 1 << s)))
+        mark("claims at rx", t0)
+        t0 = t()
+        r = challenge("inner_r", tuple(claims)) % p
+        abc, joint = [], []
+        for pr, q, c in zip(self.provers, eq_rx, claims):
+            ys = [vec(2 * pr.num_vars) for _ in range(3)]
+            for M, y in zip(pr.MT, ys):
+                M.mv(f, q.data_ptr(), y.data_ptr())
+            a = torch.empty_like(ys[0])
+            pr._axpy(ys[0], ys[1], r, a)
+            pr._axpy(a, ys[2], r * r % p, a)
+            abc.append(a)
+            joint.append((c[0] + r * c[1] + r * r * c[2]) % p)
+        mark("eval tables (transposed SpMV)", t0)
+        t0 = t()
+        r3 = pow(r, 3, p)
+        zc = [inst[0].clone() for inst in instances]
+        inner_rounds, r_y, _ = sumcheck_prove_batch(f, QUAD, [([a.data_ptr(), z.data_ptr()], ti) for a, z, ti in zip(abc, zc, T)], joint,
+                                                    [pow(r3, i, p) for i in range(N)], cb("inner"))
+        del zc, abc
+        mark("inner sum-check (batched)", t0)
+        t0 = t()
+        ry = [r_y[len(r_y) - ti:] for ti in T]
+        eval_W = []
+        for pr, (d_z, _, _), y in zip(self.provers, instances, ry):
+            q = vec(pr.num_vars)
+            eq_evals(f, y[1:], q.data_ptr())
+            eval_W.append(inner_product(f, d_z.data_ptr(), q.data_ptr(), pr.num_vars))
+        mark("eval W", t0)
+        t0 = t()
+        be = [(inst[0].data_ptr(), ti - 1, y[1:], ev) for inst, ti, y, ev in zip(instances, T, ry, eval_W)]
+        be += [(e.data_ptr(), s, x, c[3]) for e, s, x, c in zip(E, S, rx, claims)]
+        red_rounds, r_red, left, weights, joint_eval, d_joint = batch_eval_reduce(f, be, cb("batch_eval"))
+        mark("batch_eval_reduce", t0)
+        return dict(outer_rounds=outer_rounds, inner_rounds=inner_rounds, claims=claims, eval_W=eval_W, reduce_rounds=red_rounds,
+                    claims_left=left, rx=rx, ry=ry, r=r_red, weights=weights, joint_eval=joint_eval, joint=d_joint, E_padded=E)
