@@ -286,6 +286,69 @@ int lurk_batch_eval_reduce_dev(int field_id, int n_claims, const void *const *d_
                                uint8_t *round_evals, uint8_t *r_out, uint8_t *claims_left, uint8_t *weights,
                                uint8_t joint_eval[32], void *d_joint, int fmt, void *stream);
 
+/* Spartan prover context: RelaxedR1CSSNARK::prove (Nova's `compress`, src/proof/nova.rs:341-356) and
+ * BatchedRelaxedR1CSSNARK::prove (SuperNova's, supernova.rs:293-317) in one call each, from the fold context's running instance.
+ * The context is created once per circuit shape: the same CSR-over-z = (W, u, X) description as lurk_fold_config: columns
+ * < n_w + 1 + n_x, coefficients in `fmt`.  It keeps the three matrices on the device and builds there, by counting sort, the merged
+ * transpose the evaluation table needs (rows = indices of the padded z = (W | 0.. | u | X | 0..) of 2 num_vars elements, entries of
+ * A, B, C grouped in that order within a row).  num_vars = 2^log_vars = next power of two of max(n_w, n_x + 1) (at least 2);
+ * rows are padded to 2^log_rows.  joint_len = 2^max(log_rows, log_vars): the length of the joint polynomial of a plain proof.
+ * Matrices of one context are used by one call at a time. */
+typedef struct lurk_spartan_ctx lurk_spartan_ctx;
+int lurk_spartan_ctx_create(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n_rows, const uint64_t *const row_ptr[3],
+                            const uint32_t *const col[3], const uint8_t *const val[3], int fmt, lurk_spartan_ctx **out);
+void lurk_spartan_ctx_destroy(lurk_spartan_ctx *ctx);
+/* any output may be NULL */
+int lurk_spartan_ctx_info(lurk_spartan_ctx *ctx, int *field_id, int *log_rows, int *log_vars, size_t *joint_len);
+/* The transcript.  `phase` says what the message is; `round` numbers the calls of one phase.
+ *   LURK_SPARTAN_TAU         plain: rounds 0 .. log_rows - 1, empty message -> tau_i;  batched: round 0, empty -> tau
+ *                            (instance i's table is eq(tau, tau^2, tau^4, ..), PowPolynomial::evals_with_powers)
+ *   LURK_SPARTAN_OUTER_R     batched only, round 0, empty -> outer_r (instance i's coefficient outer_r^i)
+ *   LURK_SPARTAN_OUTER       each outer (cubic) sum-check round: s(0) | s(1) | s(2) | s(3) -> r_x[j]
+ *   LURK_SPARTAN_CLAIMS      round 0: Az, Bz, Cz, E at rx_i, instance after instance -> r (joint_i = Az + r Bz + r^2 Cz; batched
+ *                            coefficients (r^3)^i)
+ *   LURK_SPARTAN_INNER       each inner (quadratic) sum-check round: s(0) | s(1) | s(2) -> r_y[j]
+ *   LURK_SPARTAN_BATCH_EVAL  rounds 0 .. m + 1 of lurk_batch_eval_reduce_dev over [W_0 .. W_{n-1}, E_0 .. E_{n-1}] at
+ *                            [ry_0[1:] .., rx_0 ..]
+ * The caller absorbs the verifier key's digest and the instance U into its transcript before the call, as Arecibo does.
+ * Writes the challenge (32 bytes, `fmt`) and returns 0, or non-zero to abort the proof. */
+#define LURK_SPARTAN_TAU 0
+#define LURK_SPARTAN_OUTER_R 1
+#define LURK_SPARTAN_OUTER 2
+#define LURK_SPARTAN_CLAIMS 3
+#define LURK_SPARTAN_INNER 4
+#define LURK_SPARTAN_BATCH_EVAL 5
+typedef int (*lurk_spartan_challenge_fn)(void *user, int phase, int round, const uint8_t *message, size_t message_len,
+                                         uint8_t challenge_out[32]);
+/* Caller-owned host buffers (any may be NULL), `fmt`.  S = max log_rows, T = max log_vars + 1, m = max(S, T - 1), n instances. */
+typedef struct lurk_spartan_proof {
+    uint8_t *outer_rounds;  /* S x 4 x 32 */
+    uint8_t *r_x;           /* S x 32; instance i's point is the last log_rows_i of them */
+    uint8_t *claims;        /* n x 4 x 32: Az, Bz, Cz, E at rx_i */
+    uint8_t *inner_rounds;  /* T x 3 x 32 */
+    uint8_t *r_y;           /* T x 32; instance i's point is the last log_vars_i + 1 */
+    uint8_t *eval_W;        /* n x 32: W_i at ry_i[1:] */
+    uint8_t *reduce_rounds; /* m x 3 x 32: the reduction's sum-check */
+    uint8_t *r;             /* m x 32: the point at which the joint polynomial is opened */
+    uint8_t *claims_left;   /* 2n x 32 */
+    uint8_t *weights;       /* 2n x 32: gamma^i; the joint commitment is sum_i weights_i C_i over [comm_W_0 .., comm_E_0 ..] */
+    uint8_t *joint_eval;    /* 32 */
+} lurk_spartan_proof;
+/* RelaxedR1CSSNARK::prove followed by batch_eval_reduce over [W, E].  d_z = (W, u, X): n_w + 1 + n_x Montgomery elements, laid out as
+ * LURK_FOLD_BUF_Z1 holds them; d_E: n_rows Montgomery elements.  Both are read, never written.  d_joint (2^m elements, not overlapping
+ * d_z or d_E) receives the joint polynomial, ready for lurk_hyperkzg_prove_dev or lurk_ipa_prove_dev.  Everything runs on `stream`;
+ * the call returns when the proof is complete. */
+int lurk_spartan_prove_dev(lurk_spartan_ctx *ctx, const void *d_z, const void *d_E, lurk_spartan_challenge_fn challenge, void *user,
+                           lurk_spartan_proof *out, void *d_joint, int fmt, void *stream);
+/* BatchedRelaxedR1CSSNARK::prove over n (1..30) running instances, instance i of shape ctxs[i] (shapes may differ; one field). */
+int lurk_spartan_prove_batch_dev(int n, lurk_spartan_ctx *const *ctxs, const void *const *d_z, const void *const *d_E,
+                                 lurk_spartan_challenge_fn challenge, void *user, lurk_spartan_proof *out, void *d_joint, int fmt,
+                                 void *stream);
+/* compute_eval_table_sparse alone: d_out[j] = sum_rows eq_rx[row] (A[row][j] + r B[row][j] + r^2 C[row][j]) over the padded z's
+ * columns (2 num_vars elements); d_eq_rx: 2^log_rows Montgomery elements; r: 32 bytes in `fmt`.  For callers that schedule the
+ * primitives themselves. */
+int lurk_spartan_eval_table_dev(lurk_spartan_ctx *ctx, const void *d_eq_rx, const uint8_t r[32], void *d_out, int fmt, void *stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * S5  Fold helpers on device-resident vectors (Arecibo NIFS::prove / R1CSShape::commit_T /
  *     RelaxedR1CSWitness::fold; SURVEY.md Appendix B).  All vectors Montgomery form on the device.

@@ -25,6 +25,20 @@ pub struct lurk_msm_ctx { _private: [u8; 0] }
 #[repr(C)]
 pub struct lurk_fold_ctx { _private: [u8; 0] }
 #[repr(C)]
+pub struct lurk_spartan_ctx { _private: [u8; 0] }
+/// caller-owned host buffers of one proof (include/lurk_b200.h: lurk_spartan_proof); null = not wanted
+#[repr(C)]
+pub struct lurk_spartan_proof {
+    pub outer_rounds: *mut u8, pub r_x: *mut u8, pub claims: *mut u8, pub inner_rounds: *mut u8, pub r_y: *mut u8, pub eval_w: *mut u8,
+    pub reduce_rounds: *mut u8, pub r: *mut u8, pub claims_left: *mut u8, pub weights: *mut u8, pub joint_eval: *mut u8,
+}
+pub const LURK_SPARTAN_TAU: c_int = 0;
+pub const LURK_SPARTAN_OUTER_R: c_int = 1;
+pub const LURK_SPARTAN_OUTER: c_int = 2;
+pub const LURK_SPARTAN_CLAIMS: c_int = 3;
+pub const LURK_SPARTAN_INNER: c_int = 4;
+pub const LURK_SPARTAN_BATCH_EVAL: c_int = 5;
+#[repr(C)]
 #[derive(Clone, Copy)]
 pub struct lurk_dag_node { pub kind: u8, pub reserved: u8, pub tag: [u16; 4], pub child: [u32; 4] }
 #[repr(C)]
@@ -97,6 +111,31 @@ extern "C" {
                                       evals: *const u8, challenge: lurk_challenge_fn, user: *mut c_void, round_evals: *mut u8, r_out: *mut u8,
                                       claims_left: *mut u8, weights: *mut u8, joint_eval: *mut u8, d_joint: *mut c_void, fmt: c_int,
                                       stream: *mut c_void) -> c_int;
+    // N4 -- RelaxedR1CSSNARK::prove / BatchedRelaxedR1CSSNARK::prove in one call (src/proof/nova.rs:341-356, supernova.rs:293-317)
+    pub fn lurk_spartan_ctx_create(field_id: c_int, n_w: u64, n_x: u64, n_rows: u64, row_ptr: *const *const u64, col: *const *const u32,
+                                   val: *const *const u8, fmt: c_int, out: *mut *mut lurk_spartan_ctx) -> c_int;
+    pub fn lurk_spartan_ctx_destroy(ctx: *mut lurk_spartan_ctx);
+    pub fn lurk_spartan_ctx_info(ctx: *mut lurk_spartan_ctx, field_id: *mut c_int, log_rows: *mut c_int, log_vars: *mut c_int, joint_len: *mut usize) -> c_int;
+    pub fn lurk_spartan_prove_dev(ctx: *mut lurk_spartan_ctx, d_z: *const c_void, d_e: *const c_void, challenge: lurk_spartan_challenge_fn, user: *mut c_void,
+                                  out: *mut lurk_spartan_proof, d_joint: *mut c_void, fmt: c_int, stream: *mut c_void) -> c_int;
+    pub fn lurk_spartan_prove_batch_dev(n: c_int, ctxs: *const *mut lurk_spartan_ctx, d_z: *const *const c_void, d_e: *const *const c_void,
+                                        challenge: lurk_spartan_challenge_fn, user: *mut c_void, out: *mut lurk_spartan_proof, d_joint: *mut c_void,
+                                        fmt: c_int, stream: *mut c_void) -> c_int;
+    pub fn lurk_spartan_eval_table_dev(ctx: *mut lurk_spartan_ctx, d_eq_rx: *const c_void, r: *const u8, d_out: *mut c_void, fmt: c_int,
+                                       stream: *mut c_void) -> c_int;
+}
+/// `int (*)(void *user, int phase, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32])`: the phase-tagged
+/// transcript of the Spartan prover context (LURK_SPARTAN_*).  The caller has absorbed the vk digest and U before the call.
+pub type lurk_spartan_challenge_fn = unsafe extern "C" fn(user: *mut c_void, phase: c_int, round: c_int, message: *const u8, message_len: usize,
+                                                          challenge_out: *mut u8) -> c_int;
+pub unsafe extern "C" fn spartan_trampoline<F: FnMut(i32, i32, &[u8]) -> Option<[u8; 32]>>(user: *mut c_void, phase: c_int, round: c_int, message: *const u8,
+                                                                                          len: usize, out: *mut u8) -> c_int {
+    let f = &mut *(user as *mut F);
+    let msg = if len == 0 { &[][..] } else { std::slice::from_raw_parts(message, len) };
+    match f(phase, round, msg) {
+        Some(r) => { std::ptr::copy_nonoverlapping(r.as_ptr(), out, 32); 0 }
+        None => 1,
+    }
 }
 /// `int (*)(void *user, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32])`: the Fiat-Shamir transcript stays in
 /// Rust.  A closure is passed as `user` and trampolined, e.g. for SumcheckProof::prove_*:
@@ -173,3 +212,42 @@ impl FoldCtx {
     }
 }
 impl Drop for FoldCtx { fn drop(&mut self) { unsafe { lurk_fold_ctx_destroy(self.raw) } } }
+
+/// One circuit shape's Spartan prover key on the device (`ProverKey` of RelaxedR1CSSNARK): the matrices and their merged transpose, built
+/// on the GPU.  `prove` runs RelaxedR1CSSNARK::prove + batch_eval_reduce straight from a fold context's running instance
+/// (`lurk_fold_ctx_device_buffer(LURK_FOLD_BUF_Z1 / _E1)`), leaving the joint polynomial in `d_joint` for the EE opening.
+pub struct SpartanCtx(*mut lurk_spartan_ctx);
+unsafe impl Send for SpartanCtx {}
+impl SpartanCtx {
+    /// row_ptr / col / val: the A, B, C CSR over z = (W, u, X) as lurk_fold_config takes them (Montgomery coefficients)
+    pub fn new(field_id: c_int, n_w: u64, n_x: u64, n_rows: u64, row_ptr: [&[u64]; 3], col: [&[u32]; 3], val: [&[u8]; 3]) -> Result<Self, B200Error> {
+        let rp = [row_ptr[0].as_ptr(), row_ptr[1].as_ptr(), row_ptr[2].as_ptr()];
+        let cl = [col[0].as_ptr(), col[1].as_ptr(), col[2].as_ptr()];
+        let vl = [val[0].as_ptr(), val[1].as_ptr(), val[2].as_ptr()];
+        let mut p = std::ptr::null_mut();
+        check(unsafe { lurk_spartan_ctx_create(field_id, n_w, n_x, n_rows, rp.as_ptr(), cl.as_ptr(), vl.as_ptr(), LURK_FMT_MONTGOMERY, &mut p) })?;
+        Ok(Self(p))
+    }
+    /// (log_rows, log_vars, joint length)
+    pub fn info(&self) -> Result<(i32, i32, usize), B200Error> {
+        let (mut lr, mut lv, mut jl) = (0, 0, 0usize);
+        check(unsafe { lurk_spartan_ctx_info(self.0, std::ptr::null_mut(), &mut lr, &mut lv, &mut jl) })?;
+        Ok((lr, lv, jl))
+    }
+    /// # Safety: d_z / d_e / d_joint are device pointers of the sizes include/lurk_b200.h gives; `out`'s buffers are large enough.
+    pub unsafe fn prove<F: FnMut(i32, i32, &[u8]) -> Option<[u8; 32]>>(&mut self, d_z: *const c_void, d_e: *const c_void, transcript: &mut F,
+                                                                       out: &mut lurk_spartan_proof, d_joint: *mut c_void) -> Result<(), B200Error> {
+        check(lurk_spartan_prove_dev(self.0, d_z, d_e, spartan_trampoline::<F>, transcript as *mut F as *mut c_void, out, d_joint,
+                                     LURK_FMT_MONTGOMERY, std::ptr::null_mut()))
+    }
+    /// BatchedRelaxedR1CSSNARK::prove over one running instance per circuit index (SuperNova)
+    /// # Safety: as `prove`, per instance.
+    pub unsafe fn prove_batch<F: FnMut(i32, i32, &[u8]) -> Option<[u8; 32]>>(ctxs: &mut [&mut SpartanCtx], d_z: &[*const c_void], d_e: &[*const c_void],
+                                                                             transcript: &mut F, out: &mut lurk_spartan_proof, d_joint: *mut c_void)
+                                                                             -> Result<(), B200Error> {
+        let raw: Vec<*mut lurk_spartan_ctx> = ctxs.iter().map(|c| c.0).collect();
+        check(lurk_spartan_prove_batch_dev(raw.len() as c_int, raw.as_ptr(), d_z.as_ptr(), d_e.as_ptr(), spartan_trampoline::<F>,
+                                           transcript as *mut F as *mut c_void, out, d_joint, LURK_FMT_MONTGOMERY, std::ptr::null_mut()))
+    }
+}
+impl Drop for SpartanCtx { fn drop(&mut self) { unsafe { lurk_spartan_ctx_destroy(self.0) } } }

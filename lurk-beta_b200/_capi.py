@@ -50,6 +50,16 @@ _vp, _sz, _i = C.c_void_p, C.c_size_t, C.c_int
 # lurk_challenge_fn: int (*)(void *user, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32])
 CHALLENGE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_uint8), C.c_size_t, C.POINTER(C.c_uint8))
 SUMCHECK_QUAD, SUMCHECK_CUBIC = 0, 1
+# lurk_spartan_challenge_fn: int (*)(void *user, int phase, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32])
+SPARTAN_CHALLENGE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint8), C.c_size_t, C.POINTER(C.c_uint8))
+SPARTAN_TAU, SPARTAN_OUTER_R, SPARTAN_OUTER, SPARTAN_CLAIMS, SPARTAN_INNER, SPARTAN_BATCH_EVAL = range(6)
+
+
+class SpartanProof(C.Structure):
+    _fields_ = [(name, C.c_void_p) for name in ("outer_rounds", "r_x", "claims", "inner_rounds", "r_y", "eval_W", "reduce_rounds", "r",
+                                                 "claims_left", "weights", "joint_eval")]
+
+
 # every symbol declared in include/lurk_b200.h: name -> (restype, argtypes)
 PROTOTYPES = {
     "lurk_last_error": (C.c_char_p, []),
@@ -102,6 +112,13 @@ PROTOTYPES = {
     "lurk_ck_powers_dev": (_i, [_i, _vp, _vp, _sz, _vp, _i, _vp]),
     "lurk_hyperkzg_prove_dev": (_i, [_i, _vp, _vp, _vp, _i, CHALLENGE_FN, _vp, _vp, _vp, _vp, _i, _vp]),
     "lurk_batch_eval_reduce_dev": (_i, [_i, _i, C.POINTER(_vp), C.POINTER(_i), _vp, _vp, CHALLENGE_FN, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    "lurk_spartan_ctx_create": (_i, [_i, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _i, C.POINTER(_vp)]),
+    "lurk_spartan_ctx_destroy": (None, [_vp]),
+    "lurk_spartan_ctx_info": (_i, [_vp, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_sz)]),
+    "lurk_spartan_prove_dev": (_i, [_vp, _vp, _vp, SPARTAN_CHALLENGE_FN, _vp, C.POINTER(SpartanProof), _vp, _i, _vp]),
+    "lurk_spartan_prove_batch_dev": (_i, [_i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), SPARTAN_CHALLENGE_FN, _vp, C.POINTER(SpartanProof), _vp, _i,
+                                          _vp]),
+    "lurk_spartan_eval_table_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
     "lurk_axpy_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lurk_spmv_csr_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
     "lurk_cross_term_dev": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),

@@ -16,6 +16,7 @@
 #pragma once
 #include "msm_impl.cuh"
 #include "poseidon_api.h"
+#include "spmv3.cuh"
 
 #include <memory>
 #include <string>
@@ -33,38 +34,6 @@ static constexpr int FOLD_W_WINDOW = 17;           // window of commit(W2 - D) (
 static constexpr int FOLD_T_WINDOW = 16;           // widest window of the chain-critical commit(T)
 
 // ----------------------------------------------------------------------------- fold kernels (witness field)
-struct CsrDev {
-    const uint64_t *row_ptr;
-    const uint32_t *col;
-    const void *val;
-};
-
-// y_m = M_m z for the three R1CS matrices in one launch (blockIdx.y = matrix), one row per thread
-template <class F>
-__global__ void __launch_bounds__(256) spmv3_kernel(CsrDev A, CsrDev B, CsrDev C, size_t rows, const F *__restrict__ z, F *__restrict__ ya,
-                                                    F *__restrict__ yb, F *__restrict__ yc) {
-    const CsrDev M = blockIdx.y == 0 ? A : (blockIdx.y == 1 ? B : C);
-    F *y = blockIdx.y == 0 ? ya : (blockIdx.y == 1 ? yb : yc);
-    const F *val = (const F *)M.val;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < rows; i += (size_t)gridDim.x * blockDim.x) {
-        const uint64_t k0 = M.row_ptr[i], k1 = M.row_ptr[i + 1];
-        F acc = F::zero();
-        if (k1 - k0 == 1) {
-            acc = load_fe<F>(val + k0) * load_fe<F>(z + M.col[k0]);
-        } else if (k1 > k0) {
-            // lazy accumulation: one Montgomery reduction per group of <= 8 products
-            for (uint64_t k = k0; k < k1;) {
-                WideAcc<typename F::Params> w;
-                w.clear();
-                const uint64_t ke = k1 - k > 8 ? k + 8 : k1;
-                for (; k < ke; k++) w.mul_acc(load_fe<F>(val + k), load_fe<F>(z + M.col[k]));
-                acc = acc + w.reduce();
-            }
-        }
-        store_fe(y + i, acc);
-    }
-}
-
 // T = az1*bz2 + az2*bz1 - u1*cz2 - u2*cz1 with u1, u2 read from the device-resident z vectors
 template <class F>
 __global__ void __launch_bounds__(256) cross_term_dev_kernel(const F *__restrict__ az1, const F *__restrict__ bz1, const F *__restrict__ cz1,

@@ -439,3 +439,124 @@ class BatchedRelaxedR1CSProver:
         mark("batch_eval_reduce", t0)
         return dict(outer_rounds=outer_rounds, inner_rounds=inner_rounds, claims=claims, eval_W=eval_W, reduce_rounds=red_rounds,
                     claims_left=left, rx=rx, ry=ry, r=r_red, weights=weights, joint_eval=joint_eval, joint=d_joint, E_padded=E)
+
+
+# ------------------------------------------------------------------------------------------------ the Spartan prover context
+def _spartan_callback(challenge, p, n, batched, errors):
+    """the phase-tagged transcript of lurk_spartan_prove_*_dev mapped onto the labels and data RelaxedR1CSProver, BatchedRelaxedR1CSProver and
+    tests/batched_oracle.py use, so that one challenge(label, data) function drives every path"""
+    labels = {_capi.SPARTAN_OUTER: "outer", _capi.SPARTAN_INNER: "inner", _capi.SPARTAN_BATCH_EVAL: "batch_eval"}
+
+    def cb(user, phase, rnd, msg, msg_len, out):
+        try:
+            vals = _ints(np.frombuffer(C.string_at(msg, msg_len), dtype=np.uint8)) if msg_len else []
+            if phase == _capi.SPARTAN_TAU:
+                x = challenge("tau", n if batched else rnd)
+            elif phase == _capi.SPARTAN_OUTER_R:
+                x = challenge("outer_r", n)
+            elif phase == _capi.SPARTAN_CLAIMS:
+                claims = tuple(tuple(vals[4 * i:4 * i + 4]) for i in range(n))
+                x = challenge("inner_r", claims if batched else claims[0])
+            else:
+                x = challenge(labels[phase], (rnd, vals))
+            for i, byte in enumerate((int(x) % p).to_bytes(32, "little")):
+                out[i] = byte
+            return 0
+        except Exception as e:          # never unwind through the C frames
+            errors.append(e)
+            return 1
+    return _capi.SPARTAN_CHALLENGE_FN(cb)
+
+
+class SpartanContext:
+    """lurk_spartan_ctx: one circuit shape's matrices on the device (and their merged transpose, built there), proving RelaxedR1CSSNARK
+    from a running instance (W, u, X), E in one C-ABI call.  mats: [(row_ptr, col, val bytes canonical)] over z = (W, u, X), as
+    RelaxedR1CSProver takes them."""
+
+    def __init__(self, field_id, mats, n_w, n_x):
+        self.field, self.n_w, self.n_x = field_id, n_w, n_x
+        self.p = int.from_bytes(field_modulus(field_id), "little")
+        self.rows = len(mats[0][0]) - 1
+        keep = []
+        for rp, col, val in mats:
+            keep += [np.ascontiguousarray(rp, dtype=np.uint64), np.ascontiguousarray(col, dtype=np.uint32),
+                     np.ascontiguousarray(val, dtype=np.uint8).reshape(-1)]
+        arr = lambda k: (C.c_void_p * 3)(*[keep[3 * m + k].ctypes.data for m in range(3)])
+        ctx = C.c_void_p()
+        self._ctx = None
+        _capi.check(_capi.lib().lurk_spartan_ctx_create(field_id, n_w, n_x, self.rows, arr(0), arr(1), arr(2), _capi.FMT_CANONICAL, C.byref(ctx)))
+        self._ctx = ctx
+        lr, lv, jl = C.c_int(), C.c_int(), C.c_size_t()
+        _capi.check(_capi.lib().lurk_spartan_ctx_info(ctx, None, C.byref(lr), C.byref(lv), C.byref(jl)))
+        self.log_rows, self.log_vars, self.joint_len = lr.value, lv.value, jl.value
+        self.num_vars = 1 << self.log_vars
+
+    def close(self):
+        if self._ctx:
+            _capi.lib().lurk_spartan_ctx_destroy(self._ctx)
+            self._ctx = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def prove(self, d_z_ptr, d_E_ptr, challenge, d_joint_ptr=None, stream=0):
+        """RelaxedR1CSSNARK::prove + batch_eval_reduce([W, E]).  d_z_ptr: (W, u, X) Montgomery (LURK_FOLD_BUF_Z1's layout), d_E_ptr: `rows`
+        Montgomery elements; neither is modified.  challenge(label, data) -> int.  Returns the transcript (RelaxedR1CSProver's keys plus
+        reduce_rounds, claims_left, r, weights, joint_eval) and `joint` (the device tensor allocated here when d_joint_ptr is None)."""
+        return _spartan_prove([self], [(d_z_ptr, d_E_ptr)], challenge, d_joint_ptr, stream, batched=False)
+
+    def eval_table(self, d_eq_ptr, r, d_out_ptr, stream=0):
+        """compute_eval_table_sparse alone: d_out[j] = sum_row eq[row] (A + r B + r^2 C)[row][j] over 2 num_vars columns"""
+        _capi.check(_capi.lib().lurk_spartan_eval_table_dev(self._ctx, C.c_void_p(d_eq_ptr), _capi.np_ptr(_fe(r)), C.c_void_p(d_out_ptr),
+                                                            _capi.FMT_CANONICAL, C.c_void_p(stream)))
+
+
+def spartan_prove_batch(ctxs, instances, challenge, d_joint_ptr=None, stream=0):
+    """BatchedRelaxedR1CSSNARK::prove through lurk_spartan_prove_batch_dev.  ctxs: SpartanContext per circuit, instances: [(d_z_ptr, d_E_ptr)].
+    Returns what BatchedRelaxedR1CSProver.prove returns (without E_padded)."""
+    return _spartan_prove(ctxs, instances, challenge, d_joint_ptr, stream, batched=True)
+
+
+def _spartan_prove(ctxs, instances, challenge, d_joint_ptr, stream, batched):
+    import torch
+    n, p = len(ctxs), ctxs[0].p
+    S = [c.log_rows for c in ctxs]
+    T = [c.log_vars + 1 for c in ctxs]
+    mS, mT = max(S), max(T)
+    m = max(mS, mT - 1)
+    joint = None
+    if d_joint_ptr is None:
+        joint = torch.empty((1 << m) * 32, dtype=torch.uint8, device="cuda")
+        d_joint_ptr = joint.data_ptr()
+    bufs = dict(outer_rounds=mS * 4, r_x=mS, claims=4 * n, inner_rounds=mT * 3, r_y=mT, eval_W=n, reduce_rounds=m * 3, r=m, claims_left=2 * n,
+                weights=2 * n, joint_eval=1)
+    bufs = {k: np.zeros(max(1, v) * 32, dtype=np.uint8) for k, v in bufs.items()}
+    rec = _capi.SpartanProof(**{k: b.ctypes.data for k, b in bufs.items()})
+    errors = []
+    cb = _spartan_callback(challenge, p, n, batched, errors)
+    lib = _capi.lib()
+    if batched:
+        cs = (C.c_void_p * n)(*[c._ctx for c in ctxs])
+        zs = (C.c_void_p * n)(*[C.c_void_p(z) for z, _ in instances])
+        es = (C.c_void_p * n)(*[C.c_void_p(e) for _, e in instances])
+        rc = lib.lurk_spartan_prove_batch_dev(n, cs, zs, es, cb, None, C.byref(rec), C.c_void_p(d_joint_ptr), _capi.FMT_CANONICAL, C.c_void_p(stream))
+    else:
+        rc = lib.lurk_spartan_prove_dev(ctxs[0]._ctx, C.c_void_p(instances[0][0]), C.c_void_p(instances[0][1]), cb, None, C.byref(rec),
+                                        C.c_void_p(d_joint_ptr), _capi.FMT_CANONICAL, C.c_void_p(stream))
+    if errors:
+        raise errors[0]
+    _capi.check(rc)
+    v = {k: _ints(b) for k, b in bufs.items()}
+    r_x, r_y = v["r_x"][:mS], v["r_y"][:mT]
+    out = dict(outer_rounds=[v["outer_rounds"][4 * j:4 * j + 4] for j in range(mS)], inner_rounds=[v["inner_rounds"][3 * j:3 * j + 3] for j in range(mT)],
+               reduce_rounds=[v["reduce_rounds"][3 * j:3 * j + 3] for j in range(m)], r=v["r"][:m], claims_left=v["claims_left"][:2 * n],
+               weights=v["weights"][:2 * n], joint_eval=v["joint_eval"][0], joint=joint)
+    claims = [tuple(v["claims"][4 * i:4 * i + 4]) for i in range(n)]
+    if batched:
+        out.update(claims=claims, eval_W=v["eval_W"][:n], rx=[r_x[mS - s:] for s in S], ry=[r_y[mT - t:] for t in T])
+    else:
+        out.update(claims=claims[0], eval_W=v["eval_W"][0], rx=r_x, ry=r_y)
+    return out
