@@ -42,8 +42,10 @@ def test_digest_parity_small_batch(L, oracle, spec, field, arity, shape):
 
 @pytest.mark.parametrize("field,arity", [(0, 8), (0, 4), (2, 8), (2, 4), (1, 3), (3, 6)])
 def test_digest_parity_throughput_path(L, oracle, field, arity):
-    # large enough for the persistent one-CTA-per-SM launch shape; oracle on 8 threads takes seconds
-    n = 148 * 512 + 77
+    # large enough for the persistent one-CTA-per-SM launch shape with a second grid-stride pass (arity 3/4: 512 threads per
+    # SM, 6/8: 384); oracle on 8 threads takes seconds
+    import torch
+    n = torch.cuda.get_device_properties(0).multi_processor_count * 512 + 77
     pre = random_elements(field, n * arity, seed=55 + field + arity)
     got = L.PoseidonCache(field).hash_batch_bytes(arity, pre)
     want = oracle.poseidon_hash_batch(field, arity, pre, mode=1, nthreads=8)
