@@ -221,7 +221,9 @@ int lurk_shake256(const uint8_t *in, size_t in_len, uint8_t *out, size_t out_len
  *     EqPolynomial::evals and the inner product behind MultilinearPolynomial::evaluate.  The Fiat-Shamir transcript (Keccak256Transcript) stays on the caller's side:
  *     every round passes its message to `challenge` and receives the verifier's challenge.  Polynomials: 2^num_rounds elements,
  *     Montgomery form, index bit (num_rounds - 1) = the first variable (bound first), as in Arecibo's MultilinearPolynomial.
- *     Not here: the transcript, proof (de)serialisation, the verifiers (HyperKZG's pairing check) -- CPU / third-party protocol code.
+ *     The verifier's data-parallel parts are here too: the matrix evaluations of RelaxedR1CSSNARK::verify and the tensor MSM of
+ *     InnerProductArgument::verify.  Not here: the transcript, proof (de)serialisation, HyperKZG's pairing check -- CPU / third-party
+ *     protocol code.
  * ------------------------------------------------------------------------------------------------- */
 /* message: the round's prover message in `fmt` -- sum-check: s(0) | s(1) | s(2) [| s(3)] (32 bytes each; Arecibo absorbs the
  * compressed form, i.e. the coefficients without the linear one: the caller converts);  IPA: L | R as 96-byte points.
@@ -261,6 +263,15 @@ int lurk_ipa_fold_bases_dev(int curve_id, void *d_bases_mont, size_t n, const ui
 int lurk_ipa_prove_dev(int curve_id, lurk_msm_ctx *ck, const uint8_t ck_c[64], void *d_a, void *d_b, int log_n,
                        lurk_challenge_fn challenge, void *user, uint8_t *L_out, uint8_t *R_out, uint8_t a_final[32], uint8_t b_final[32],
                        int fmt, void *stream);
+/* InnerProductArgument::verify for the claim <a, b> = c with comm = commit(a): per round r_j = challenge(j, L_j | R_j) (as in the prover),
+ * s[i] = prod_j (bit_j(i) ? r_j : 1 / r_j) (bit 0 = the top bit of i), ck_hat = commit(ck, s) over 2^log_n bases of `ck` (NOT consumed),
+ * b_hat = <b, s>; accepted iff a_final ck_hat + a_final b_hat ck_c == comm + c ck_c + sum_j (r_j^2 L_j + r_j^-2 R_j).  d_b: 2^log_n
+ * Montgomery elements on the device (not modified); ck_c: 64 bytes affine; comm, L, R (log_n x 96), ck_hat_out: 96-byte points; scalars 32
+ * bytes; all in `fmt`.  Points off the curve and values >= p are LURK_ERR_RANGE; a failed check is LURK_OK with *accepted = 0.
+ * ck_hat_out / b_hat_out may be NULL.  Synchronous. */
+int lurk_ipa_verify_dev(int curve_id, lurk_msm_ctx *ck, const uint8_t ck_c[64], const uint8_t comm[96], const uint8_t c[32], const void *d_b,
+                        int log_n, const uint8_t *L, const uint8_t *R, const uint8_t a_final[32], lurk_challenge_fn challenge, void *user,
+                        int *accepted, uint8_t ck_hat_out[96], uint8_t b_hat_out[32], int fmt, void *stream);
 /* provider::hyperkzg::EvaluationEngine::prove (the opening argument of the primary BN256 circuit, EE1 in src/proof/nova.rs:65-71):
  * d_poly = 2^num_vars evaluations (Montgomery, not modified), point = num_vars elements (host, `fmt`), ck = a context on the KZG key
  * (>= 2^num_vars bases).  Phase 1: P_{i+1}[j] = P_i[2j] + x_{l-1-i} (P_i[2j+1] - P_i[2j]) and com_i = commit(P_i), i = 1..l-1;
@@ -348,6 +359,31 @@ int lurk_spartan_prove_batch_dev(int n, lurk_spartan_ctx *const *ctxs, const voi
  * columns (2 num_vars elements); d_eq_rx: 2^log_rows Montgomery elements; r: 32 bytes in `fmt`.  For callers that schedule the
  * primitives themselves. */
 int lurk_spartan_eval_table_dev(lurk_spartan_ctx *ctx, const void *d_eq_rx, const uint8_t r[32], void *d_out, int fmt, void *stream);
+/* The verifier's side (RelaxedR1CSSNARK::verify, BatchedRelaxedR1CSSNARK::verify: CompressedSNARK::verify, src/proof/nova.rs:358-373).
+ * lurk_spartan_matrix_evals_dev: the multilinear extensions of A, B, C at (r_x, r_y) -- r_x: log_rows elements, r_y: log_vars + 1
+ * elements over the padded z, both `fmt`; out = A | B | C (3 x 32, `fmt`).  One pass over the context's non-zeros with eq(r_x) and
+ * eq(r_y) looked up in product-tensor tables in shared memory: no O(rows) or O(columns) scratch.  Synchronous. */
+int lurk_spartan_matrix_evals_dev(lurk_spartan_ctx *ctx, const uint8_t *r_x, const uint8_t *r_y, uint8_t out[96], int fmt, void *stream);
+/* Round polynomials of a proof handed to the verifiers:
+ *   LURK_SPARTAN_ROUNDS_EVALS       s(0) | s(1) | .. | s(d) per round, as lurk_spartan_prove_dev writes them (outer S x 4, inner T x 3,
+ *                                   reduction m x 3 elements); each round must sum to the running claim.
+ *   LURK_SPARTAN_ROUNDS_COMPRESSED  Arecibo's CompressedUniPoly: every coefficient but the linear one, constant first (outer S x 3,
+ *                                   inner T x 2, reduction m x 2 elements); the linear one is recovered from the running claim.
+ * In both cases `challenge` receives the evaluations s(0) | .. | s(d), exactly the messages of the prover. */
+#define LURK_SPARTAN_ROUNDS_EVALS 0
+#define LURK_SPARTAN_ROUNDS_COMPRESSED 1
+/* RelaxedR1CSSNARK::verify up to the opening, then the verifier of batch_eval_reduce over [W, E] at [r_y[1:], r_x].  u (32 bytes) and
+ * X (n_x x 32 bytes) are the instance's public values, in `fmt`.  Reads outer_rounds, claims, inner_rounds, eval_W, reduce_rounds and
+ * claims_left of `proof`; when the proof is accepted, writes r_x, r_y, r, weights and joint_eval wherever they are non-NULL (the bytes the
+ * prover wrote).  `challenge` is called with the phases, rounds and messages of lurk_spartan_prove_dev, in the same order, so one transcript
+ * drives both.  What remains for the caller is the opening: the joint commitment sum_i weights_i C_i over [comm_W, comm_E] at r has value
+ * joint_eval.  A proof that fails a check is not an error: LURK_OK with *accepted = 0.  Values >= p are LURK_ERR_RANGE. */
+int lurk_spartan_verify(lurk_spartan_ctx *ctx, const uint8_t u[32], const uint8_t *X, lurk_spartan_proof *proof, int rounds_fmt,
+                        lurk_spartan_challenge_fn challenge, void *user, int *accepted, int fmt, void *stream);
+/* BatchedRelaxedR1CSSNARK::verify over n (1..30) instances of shapes ctxs[i] (distinct contexts, one field): u = n x 32 bytes, X[i] =
+ * instance i's n_x_i x 32 bytes.  One matrix-evaluation launch per instance and one synchronisation. */
+int lurk_spartan_verify_batch(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u, const uint8_t *const *X, lurk_spartan_proof *proof,
+                              int rounds_fmt, lurk_spartan_challenge_fn challenge, void *user, int *accepted, int fmt, void *stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * S5  Fold helpers on device-resident vectors (Arecibo NIFS::prove / R1CSShape::commit_T /

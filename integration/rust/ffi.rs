@@ -123,7 +123,19 @@ extern "C" {
                                         fmt: c_int, stream: *mut c_void) -> c_int;
     pub fn lurk_spartan_eval_table_dev(ctx: *mut lurk_spartan_ctx, d_eq_rx: *const c_void, r: *const u8, d_out: *mut c_void, fmt: c_int,
                                        stream: *mut c_void) -> c_int;
+    // N4 -- the data-parallel parts of CompressedSNARK::verify (src/proof/nova.rs:358-373)
+    pub fn lurk_spartan_matrix_evals_dev(ctx: *mut lurk_spartan_ctx, r_x: *const u8, r_y: *const u8, out: *mut u8, fmt: c_int, stream: *mut c_void) -> c_int;
+    pub fn lurk_spartan_verify(ctx: *mut lurk_spartan_ctx, u: *const u8, x: *const u8, proof: *mut lurk_spartan_proof, rounds_fmt: c_int,
+                               challenge: lurk_spartan_challenge_fn, user: *mut c_void, accepted: *mut c_int, fmt: c_int, stream: *mut c_void) -> c_int;
+    pub fn lurk_spartan_verify_batch(n: c_int, ctxs: *const *mut lurk_spartan_ctx, u: *const u8, x: *const *const u8, proof: *mut lurk_spartan_proof,
+                                     rounds_fmt: c_int, challenge: lurk_spartan_challenge_fn, user: *mut c_void, accepted: *mut c_int, fmt: c_int,
+                                     stream: *mut c_void) -> c_int;
+    pub fn lurk_ipa_verify_dev(curve_id: c_int, ck: *mut lurk_msm_ctx, ck_c: *const u8, comm: *const u8, c: *const u8, d_b: *const c_void, log_n: c_int,
+                               l: *const u8, r: *const u8, a_final: *const u8, challenge: lurk_challenge_fn, user: *mut c_void, accepted: *mut c_int,
+                               ck_hat_out: *mut u8, b_hat_out: *mut u8, fmt: c_int, stream: *mut c_void) -> c_int;
 }
+pub const LURK_SPARTAN_ROUNDS_EVALS: c_int = 0;
+pub const LURK_SPARTAN_ROUNDS_COMPRESSED: c_int = 1;
 /// `int (*)(void *user, int phase, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32])`: the phase-tagged
 /// transcript of the Spartan prover context (LURK_SPARTAN_*).  The caller has absorbed the vk digest and U before the call.
 pub type lurk_spartan_challenge_fn = unsafe extern "C" fn(user: *mut c_void, phase: c_int, round: c_int, message: *const u8, message_len: usize,
@@ -249,5 +261,40 @@ impl SpartanCtx {
         check(lurk_spartan_prove_batch_dev(raw.len() as c_int, raw.as_ptr(), d_z.as_ptr(), d_e.as_ptr(), spartan_trampoline::<F>,
                                            transcript as *mut F as *mut c_void, out, d_joint, LURK_FMT_MONTGOMERY, std::ptr::null_mut()))
     }
+    /// RelaxedR1CSSNARK::verify up to the opening, from Arecibo's proof fields with their compressed round polynomials; on acceptance `proof`'s
+    /// r / weights / joint_eval say which opening remains.  Ok(false) = rejected.
+    /// # Safety: `proof`'s buffers have the sizes include/lurk_b200.h gives; u is 32 bytes, x n_x x 32 bytes (Montgomery).
+    pub unsafe fn verify<F: FnMut(i32, i32, &[u8]) -> Option<[u8; 32]>>(&mut self, u: &[u8], x: &[u8], transcript: &mut F, proof: &mut lurk_spartan_proof)
+                                                                        -> Result<bool, B200Error> {
+        let mut accepted: c_int = 0;
+        check(lurk_spartan_verify(self.0, u.as_ptr(), x.as_ptr(), proof, LURK_SPARTAN_ROUNDS_COMPRESSED, spartan_trampoline::<F>,
+                                  transcript as *mut F as *mut c_void, &mut accepted, LURK_FMT_MONTGOMERY, std::ptr::null_mut()))?;
+        Ok(accepted != 0)
+    }
+    /// BatchedRelaxedR1CSSNARK::verify (SuperNova): u = n x 32 bytes, x[i] = instance i's public values.
+    /// # Safety: as `verify`, per instance.
+    pub unsafe fn verify_batch<F: FnMut(i32, i32, &[u8]) -> Option<[u8; 32]>>(ctxs: &mut [&mut SpartanCtx], u: &[u8], x: &[&[u8]], transcript: &mut F,
+                                                                              proof: &mut lurk_spartan_proof) -> Result<bool, B200Error> {
+        let raw: Vec<*mut lurk_spartan_ctx> = ctxs.iter().map(|c| c.0).collect();
+        let xs: Vec<*const u8> = x.iter().map(|v| v.as_ptr()).collect();
+        let mut accepted: c_int = 0;
+        check(lurk_spartan_verify_batch(raw.len() as c_int, raw.as_ptr(), u.as_ptr(), xs.as_ptr(), proof, LURK_SPARTAN_ROUNDS_COMPRESSED,
+                                        spartan_trampoline::<F>, transcript as *mut F as *mut c_void, &mut accepted, LURK_FMT_MONTGOMERY,
+                                        std::ptr::null_mut()))?;
+        Ok(accepted != 0)
+    }
+}
+
+/// InnerProductArgument::verify (EE2, and EE1 on Pallas): `comm` = the joint commitment, `c` = joint_eval, `d_b` = eq(r) on the device (2^log_n
+/// Montgomery elements), `l` / `r` = the proof's L_vec / R_vec as 96-byte points.  The key context is not consumed.  Ok(false) = rejected.
+/// # Safety: `d_b` is a device pointer of 2^log_n elements; `l` / `r` hold log_n points each.
+pub unsafe fn ipa_verify<F: FnMut(i32, &[u8]) -> Option<[u8; 32]>>(curve_id: c_int, ck: &MsmCtx, ck_c: &[u8; 64], comm: &[u8; 96], c: &[u8; 32],
+                                                                   d_b: *const c_void, log_n: i32, l: &[u8], r: &[u8], a_final: &[u8; 32],
+                                                                   transcript: &mut F) -> Result<bool, B200Error> {
+    let mut accepted: c_int = 0;
+    check(lurk_ipa_verify_dev(curve_id, ck.raw(), ck_c.as_ptr(), comm.as_ptr(), c.as_ptr(), d_b, log_n, l.as_ptr(), r.as_ptr(), a_final.as_ptr(),
+                              challenge_trampoline::<F>, transcript as *mut F as *mut c_void, &mut accepted, std::ptr::null_mut(),
+                              std::ptr::null_mut(), LURK_FMT_MONTGOMERY, std::ptr::null_mut()))?;
+    Ok(accepted != 0)
 }
 impl Drop for SpartanCtx { fn drop(&mut self) { unsafe { lurk_spartan_ctx_destroy(self.0) } } }

@@ -53,6 +53,7 @@ SUMCHECK_QUAD, SUMCHECK_CUBIC = 0, 1
 # lurk_spartan_challenge_fn: int (*)(void *user, int phase, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32])
 SPARTAN_CHALLENGE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint8), C.c_size_t, C.POINTER(C.c_uint8))
 SPARTAN_TAU, SPARTAN_OUTER_R, SPARTAN_OUTER, SPARTAN_CLAIMS, SPARTAN_INNER, SPARTAN_BATCH_EVAL = range(6)
+SPARTAN_ROUNDS_EVALS, SPARTAN_ROUNDS_COMPRESSED = 0, 1
 
 
 class SpartanProof(C.Structure):
@@ -119,6 +120,11 @@ PROTOTYPES = {
     "lurk_spartan_prove_batch_dev": (_i, [_i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), SPARTAN_CHALLENGE_FN, _vp, C.POINTER(SpartanProof), _vp, _i,
                                           _vp]),
     "lurk_spartan_eval_table_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
+    "lurk_spartan_matrix_evals_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp]),
+    "lurk_spartan_verify": (_i, [_vp, _vp, _vp, C.POINTER(SpartanProof), _i, SPARTAN_CHALLENGE_FN, _vp, C.POINTER(_i), _i, _vp]),
+    "lurk_spartan_verify_batch": (_i, [_i, C.POINTER(_vp), _vp, C.POINTER(_vp), C.POINTER(SpartanProof), _i, SPARTAN_CHALLENGE_FN, _vp, C.POINTER(_i),
+                                       _i, _vp]),
+    "lurk_ipa_verify_dev": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, CHALLENGE_FN, _vp, C.POINTER(_i), _vp, _vp, _i, _vp]),
     "lurk_axpy_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lurk_spmv_csr_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),
     "lurk_cross_term_dev": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),

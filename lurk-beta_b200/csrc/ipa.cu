@@ -3,11 +3,14 @@
 // (reference src/proof/nova.rs:57-71, 341-356).  Split from sumcheck.cu to keep the two translation units' nvcc time apart.
 //   ipa_fold_scalars / _bases    a' = x a_lo + y a_hi;  G' = x G_lo + y G_hi (interleaved double-and-add, uniform branches).
 //   ipa_weighted / weights_update the prover's own path: commitments of a round as Pippenger passes over the fixed key.
+//   ipa_s_kernel                 the verifier's s = tensor of (1 / r_j, r_j) and <b, s> in one pass, for ck_hat = commit(ck, s).
 #include "common.cuh"
 #include "sumcheck.cuh"
 #include "sc_scratch.cuh"
+#include "tensor.cuh"
 
 #include <algorithm>
+#include <thread>
 #include <vector>
 
 namespace lurk {
@@ -182,6 +185,182 @@ static int ipa_prove(lurk_msm_ctx *ck, const uint8_t *gc_bytes, void *d_a, void 
     return LURK_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ the verifier
+// s[i] = prod_j (bit_j(i) ? r_j : 1 / r_j) -- the prover's key weights after its last round -- from product-tensor tables in shared memory
+// (tensor.cuh), written for the commitment ck_hat = commit(ck, s), and b_hat = <b, s> accumulated in the same pass.
+template <class F>
+struct IpaSArgs {
+    TensorSpec<F> t;
+    const F *b;
+    F *s;
+    size_t n;
+    F *partial;
+    unsigned *counter;
+    F *result;
+};
+
+template <class F>
+__global__ void __launch_bounds__(256) ipa_s_kernel(const __grid_constant__ IpaSArgs<F> a) {
+    extern __shared__ uint4 ipa_tensor_smem[];
+    F *tab = reinterpret_cast<F *>(ipa_tensor_smem);
+    const int groups = tensor_groups(a.t.l);
+    tensor_build(a.t, tab);
+    __syncthreads();
+    F acc[1] = {F::zero()};
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += (size_t)gridDim.x * blockDim.x) {
+        const F v = tensor_at(tab, groups, i);
+        store_fe(a.s + i, v);
+        acc[0] += load_fe<F>(a.b + i) * v;
+    }
+    grid_sum<F, 1>(acc, a.partial, a.counter, a.result);
+}
+
+// a 96-byte point x | y | z of the header's convention (z = 1, or x = y = z = 0 for the identity), on the curve y^2 = x^3 + b
+template <class Fb>
+static bool point_in(const uint8_t *in, int fmt, const Fb &b, XYZZ<Fb> &out) {
+    Affine<Fb> p;
+    Fb z;
+    if (!fe_in(in, fmt, p.x) || !fe_in(in + 32, fmt, p.y) || !fe_in(in + 64, fmt, z)) return false;
+    if (z.is_zero()) { out = XYZZ<Fb>::identity(); return p.x.is_zero() && p.y.is_zero(); }
+    if (z != Fb::one() || p.y.sqr() != p.x.sqr() * p.x + b) return false;
+    out = XYZZ<Fb>::from_affine(p);
+    return true;
+}
+
+// sum_{lo <= k < hi} scalars[k] P_k on the host: Straus, 4-bit windows, the 252 doublings shared by all terms of the range
+template <class Fb, class Fs>
+static XYZZ<Fb> host_straus(const std::vector<XYZZ<Fb>> &pts, const std::vector<Fs> &scalars, size_t lo, size_t hi) {
+    const size_t n = hi - lo;
+    std::vector<XYZZ<Fb>> tab(n * 16);
+    std::vector<Fs> k(n);
+    for (size_t i = 0; i < n; i++) {
+        k[i] = scalars[lo + i].to_canonical();
+        tab[16 * i] = XYZZ<Fb>::identity();
+        for (int d = 1; d < 16; d++) { tab[16 * i + d] = tab[16 * i + d - 1]; tab[16 * i + d].add(pts[lo + i]); }
+    }
+    XYZZ<Fb> acc = XYZZ<Fb>::identity();
+    for (int w = 63; w >= 0; w--) {
+        for (int t = 0; t < 4; t++) acc = acc.dbl();
+        for (size_t i = 0; i < n; i++) {
+            const uint32_t d = (k[i].v[w >> 3] >> (4 * (w & 7))) & 15u;
+            if (d) acc.add(tab[16 * i + d]);
+        }
+    }
+    return acc;
+}
+
+// sum_k scalars[k] P_k: the terms split over host threads (the window additions dominate: 64 per term against 256 shared doublings)
+template <class Fb, class Fs>
+static XYZZ<Fb> host_msm(const std::vector<XYZZ<Fb>> &pts, const std::vector<Fs> &scalars) {
+    const size_t n = pts.size();
+    const size_t parts = std::max<size_t>(1, std::min<size_t>({(n + 3) / 4, 16, std::max(1u, std::thread::hardware_concurrency())}));
+    std::vector<XYZZ<Fb>> partial(parts);
+    std::vector<std::thread> pool;
+    for (size_t t = 1; t < parts; t++)
+        pool.emplace_back([&, t] { partial[t] = host_straus(pts, scalars, n * t / parts, n * (t + 1) / parts); });
+    partial[0] = host_straus(pts, scalars, 0, n / parts);
+    for (std::thread &th : pool) th.join();
+    XYZZ<Fb> acc = partial[0];
+    for (size_t t = 1; t < parts; t++) acc.add(partial[t]);
+    return acc;
+}
+
+template <class Fb>
+static bool same_point(const XYZZ<Fb> &p, const XYZZ<Fb> &q) {
+    if (p.is_identity() || q.is_identity()) return p.is_identity() && q.is_identity();
+    const Affine<Fb> a = p.to_affine(), b = q.to_affine();
+    return a.x == b.x && a.y == b.y;
+}
+
+template <class C>
+static int ipa_verify(lurk_msm_ctx *ck, const uint8_t *gc_bytes, const uint8_t *comm_bytes, const uint8_t *c_bytes, const void *d_b, int log_n,
+                      const uint8_t *L, const uint8_t *R, const uint8_t *a_bytes, lurk_challenge_fn challenge, void *user, int *accepted,
+                      uint8_t *ck_hat_out, uint8_t *b_hat_out, int fmt, cudaStream_t s) {
+    using Fb = typename C::Base;
+    using Fs = typename C::Scalar;
+    *accepted = 0;
+    const Affine<Fb> g = curve_generator<C>();
+    const Fb b = g.y.sqr() - g.x.sqr() * g.x;
+    uint8_t gc3[96] = {0};
+    memcpy(gc3, gc_bytes, 64);
+    bool gc_identity = true;
+    for (int i = 0; i < 64; i++) gc_identity &= gc_bytes[i] == 0;
+    if (!gc_identity) fe_out(Fb::one(), fmt, gc3 + 64);
+    XYZZ<Fb> gc, comm;
+    if (!point_in(gc3, fmt, b, gc)) { set_error("ck_c is not a reduced point on the curve"); return LURK_ERR_RANGE; }
+    if (!point_in(comm_bytes, fmt, b, comm)) { set_error("comm is not a point of the header's form on the curve"); return LURK_ERR_RANGE; }
+    Fs c, a_hat;
+    if (!fe_in(c_bytes, fmt, c) || !fe_in(a_bytes, fmt, a_hat)) { set_error("c or a_final is not reduced"); return LURK_ERR_RANGE; }
+    // every point is checked before the first transcript call: pts = comm, ck_c, L_0, R_0, L_1, R_1, ..
+    std::vector<XYZZ<Fb>> pts{comm, gc};
+    for (int j = 0; j < log_n; j++) {
+        XYZZ<Fb> Lj, Rj;
+        if (!point_in(L + 96 * (size_t)j, fmt, b, Lj) || !point_in(R + 96 * (size_t)j, fmt, b, Rj)) {
+            set_error("L or R of round %d is not a point of the header's form on the curve", j);
+            return LURK_ERR_RANGE;
+        }
+        pts.push_back(Lj);
+        pts.push_back(Rj);
+    }
+    std::vector<Fs> sc(pts.size());
+    sc[0] = Fs::one();
+    TensorSpec<Fs> t;
+    memset(&t, 0, sizeof t);
+    t.l = log_n;
+    for (int j = 0; j < log_n; j++) {
+        uint8_t lr[192], rb[32];
+        memcpy(lr, L + 96 * (size_t)j, 96);
+        memcpy(lr + 96, R + 96 * (size_t)j, 96);
+        const int rc = challenge(user, j, lr, 192, rb);
+        if (rc != 0) { set_error("challenge callback failed in round %d (%d)", j, rc); return LURK_ERR_ARG; }
+        Fs r;
+        if (!fe_in(rb, fmt, r) || r.is_zero()) { set_error("challenge of round %d is zero or not reduced", j); return LURK_ERR_RANGE; }
+        const Fs r_inv = r.inv();
+        t.hi[j] = r;
+        t.lo[j] = r_inv;
+        sc[2 + 2 * j] = r * r;
+        sc[3 + 2 * j] = r_inv * r_inv;
+    }
+    // s and b_hat, then ck_hat = commit(ck, s) on the key context.  b_hat is read as soon as the s pass ends, so that the host's side of
+    // the check, Q = comm + (c - a_hat b_hat) ck_c + sum_j (r_j^2 L_j + r_j^-2 R_j), is computed while the commitment runs; after it only
+    // a_hat ck_hat == Q is left.
+    const size_t n = (size_t)1 << log_n;
+    StreamBuf sbuf;
+    LURK_TRY(sbuf.alloc(n * sizeof(Fs), s));
+    ScScratch<Fs> scr;
+    LURK_TRY(scr.init(s));
+    IpaSArgs<Fs> a;
+    a.t = t;
+    a.b = static_cast<const Fs *>(d_b);
+    a.s = static_cast<Fs *>(sbuf.p);
+    a.n = n;
+    a.partial = scr.partial;
+    a.counter = scr.counter;
+    a.result = scr.result;
+    const size_t smem = (size_t)tensor_groups(log_n) * TENSOR_GROUP * sizeof(Fs);
+    LURK_CUDA_TRY(cudaFuncSetAttribute(ipa_s_kernel<Fs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ipa_s_kernel<Fs><<<sc_grid(n, 256), 256, smem, s>>>(a);
+    LURK_CUDA_TRY(cudaGetLastError());
+    EventGuard s_done;
+    LURK_TRY(s_done.create());
+    LURK_CUDA_TRY(cudaEventRecord(s_done.e, s));
+    LURK_TRY(lurk_msm_ctx_launch_dev(ck, sbuf.p, n, LURK_FMT_MONTGOMERY, s));
+    LURK_CUDA_TRY(cudaEventSynchronize(s_done.e));
+    const Fs b_hat = *static_cast<const Fs *>(scr.pinned);
+    sc[1] = c - a_hat * b_hat;
+    const XYZZ<Fb> q = host_msm(pts, sc);
+    uint8_t hat[96];
+    LURK_TRY(lurk_msm_ctx_finish(ck, hat));
+    XYZZ<Fb> ck_hat = XYZZ<Fb>::identity();
+    Fb z;
+    memcpy(z.v, hat + 64, 32);
+    if (!z.is_zero()) { Affine<Fb> p; memcpy(p.x.v, hat, 32); memcpy(p.y.v, hat + 32, 32); ck_hat = XYZZ<Fb>::from_affine(p); }
+    *accepted = same_point(host_msm(std::vector<XYZZ<Fb>>{ck_hat}, std::vector<Fs>{a_hat}), q) ? 1 : 0;
+    if (ck_hat_out) point_to_bytes_fmt(ck_hat, fmt, ck_hat_out);
+    if (b_hat_out) fe_out(b_hat, fmt, b_hat_out);
+    return LURK_OK;
+}
+
 }  // namespace lurk
 
 using namespace lurk;
@@ -237,6 +416,27 @@ int lurk_ipa_prove_dev(int curve_id, lurk_msm_ctx *ck, const uint8_t ck_c[64], v
     return dispatch_curve(curve_id, [&](auto c) {
         return ipa_prove<decltype(c)>(ck, ck_c, d_a, d_b, log_n, challenge, user, L_out, R_out, a_final, b_final, fmt,
                                       static_cast<cudaStream_t>(stream));
+    });
+}
+
+int lurk_ipa_verify_dev(int curve_id, lurk_msm_ctx *ck, const uint8_t ck_c[64], const uint8_t comm[96], const uint8_t c[32], const void *d_b,
+                        int log_n, const uint8_t *L, const uint8_t *R, const uint8_t a_final[32], lurk_challenge_fn challenge, void *user,
+                        int *accepted, uint8_t ck_hat_out[96], uint8_t b_hat_out[32], int fmt, void *stream) {
+    if (!ck || !ck_c || !comm || !c || !d_b || !a_final || !challenge || !accepted) { set_error("null argument"); return LURK_ERR_ARG; }
+    if (log_n < 0 || log_n > 30) { set_error("bad log_n %d", log_n); return LURK_ERR_ARG; }
+    if (log_n > 0 && (!L || !R)) { set_error("null L / R"); return LURK_ERR_ARG; }
+    if (fmt != LURK_FMT_CANONICAL && fmt != LURK_FMT_MONTGOMERY) { set_error("bad format %d", fmt); return LURK_ERR_ARG; }
+    LURK_TRY(require_gpu());
+    int ck_curve = -1;
+    size_t ck_n = 0;
+    LURK_TRY(lurk_msm_ctx_info(ck, &ck_curve, &ck_n));
+    if (ck_curve != curve_id || ck_n < ((size_t)1 << log_n)) {
+        set_error("commitment key: curve %d with %zu bases, need curve %d with >= 2^%d", ck_curve, ck_n, curve_id, log_n);
+        return LURK_ERR_ARG;
+    }
+    return dispatch_curve(curve_id, [&](auto cv) {
+        return ipa_verify<decltype(cv)>(ck, ck_c, comm, c, d_b, log_n, L, R, a_final, challenge, user, accepted, ck_hat_out, b_hat_out, fmt,
+                                        static_cast<cudaStream_t>(stream));
     });
 }
 

@@ -9,6 +9,13 @@ namespace lurk {
 struct StreamGuard { cudaStream_t s = nullptr; ~StreamGuard() { if (s) cudaStreamDestroy(s); } int create() { LURK_CUDA_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); return LURK_OK; } };
 struct EventGuard { cudaEvent_t e = nullptr; ~EventGuard() { if (e) cudaEventDestroy(e); } int create() { LURK_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); return LURK_OK; } };
 struct MsmCloneGuard { lurk_msm_ctx *c = nullptr; ~MsmCloneGuard() { if (c) lurk_msm_ctx_destroy(c); } };
+// stream-ordered scratch, freed (in stream order) when the call returns
+struct StreamBuf {
+    void *p = nullptr;
+    cudaStream_t s = nullptr;
+    ~StreamBuf() { if (p) cudaFreeAsync(p, s); }
+    int alloc(size_t bytes, cudaStream_t st) { s = st; LURK_CUDA_TRY(cudaMallocAsync(&p, bytes ? bytes : 16, st)); return LURK_OK; }
+};
 
 static inline int sc_grid(size_t n, int block) {
     size_t want = (n + block - 1) / block;

@@ -15,8 +15,11 @@
 //                              16 entries cost: a row cut by a chunk boundary leaves one partial per chunk it touches, the last chunk
 //                              to arrive (a per-row ticket) sums them with its whole warp.  Empty rows are written in a separate
 //                              row-indexed sweep of the same threads.
+//   sp_matrix_eval_kernel      the verifier's (A, B, C)(r_x, r_y) in one launch: the row-major CSRs streamed once, eq(r_x) and eq(r_y)
+//                              looked up in product-tensor tables in shared memory (tensor.cuh).
 #include "sumcheck_impl.cuh"
 #include "spmv3.cuh"
+#include "tensor.cuh"
 
 namespace lurk {
 
@@ -203,6 +206,66 @@ __global__ void __launch_bounds__(256) sp_eval_table_kernel(const __grid_constan
     }
 }
 
+// ------------------------------------------------------------------------------------------------ verify-time kernel
+// (A(rx, ry), B(rx, ry), C(rx, ry)) = sum over the non-zeros of M of eq(rx, row) M[row][col] eq(ry, col') with col' the column in the
+// padded z.  The three row-major CSRs are one range of non-zeros (A | B | C) cut into SP_CHUNK-element chunks, so a row of 2000 entries
+// is spread over many threads; a cut row needs no fix-up because the partial sums only add.  eq(rx) and eq(ry) come from product-tensor
+// tables built per CTA in shared memory (tensor.cuh): nothing of O(rows) or O(columns) is read or written besides the CSR itself.
+template <class F>
+struct SpMatArgs {
+    const uint64_t *rp[3];
+    const uint32_t *col[3];
+    const F *val[3];
+    uint64_t off[4];             // first non-zero of A, B, C in the joint range; off[3] = total
+    uint64_t chunks;             // ceil(off[3] / SP_CHUNK)
+    size_t rows;
+    uint64_t n_w, num_vars;
+    TensorSpec<F> x, y;          // eq(rx) over the log_rows row bits, eq(ry) over the log_vars + 1 bits of the padded z
+    F *partial;
+    unsigned *counter;
+    F *result;                   // 3 elements
+};
+
+template <class F>
+__global__ void __launch_bounds__(256, 2) sp_matrix_eval_kernel(const __grid_constant__ SpMatArgs<F> a) {
+    extern __shared__ uint4 sp_tensor_smem[];
+    F *tx = reinterpret_cast<F *>(sp_tensor_smem);
+    const int gx = tensor_groups(a.x.l), gy = tensor_groups(a.y.l);
+    F *ty = tx + gx * TENSOR_GROUP;
+    tensor_build(a.x, tx);
+    tensor_build(a.y, ty);
+    __syncthreads();
+    F acc[3] = {F::zero(), F::zero(), F::zero()};
+    for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < a.chunks; c += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t c1 = min(a.off[3], (c + 1) * SP_CHUNK);
+        uint64_t e = c * SP_CHUNK;
+        while (e < c1) {
+            const int m = (e >= a.off[1]) + (e >= a.off[2]);        // empty matrices have off[m] = off[m + 1] and are skipped
+            const uint64_t base = a.off[m], stop = min(c1, a.off[m + 1]) - base;
+            const uint64_t *rp = m == 0 ? a.rp[0] : m == 1 ? a.rp[1] : a.rp[2];
+            const uint32_t *col = m == 0 ? a.col[0] : m == 1 ? a.col[1] : a.col[2];
+            const F *val = m == 0 ? a.val[0] : m == 1 ? a.val[1] : a.val[2];
+            uint64_t k = e - base;
+            size_t j = sp_row_of(rp, a.rows, k);
+            F sum = F::zero();
+            while (true) {
+                const uint64_t end = min(rp[j + 1], stop);
+                F row = F::zero();
+                for (; k < end; k++) row += load_fe<F>(val + k) * tensor_at(ty, gy, sp_col(col[k], a.n_w, a.num_vars));
+                sum += tensor_at(tx, gx, j) * row;
+                if (k >= stop) break;
+                j++;
+                if (rp[j + 1] == k) j = sp_row_of(rp, a.rows, k);      // skip a run of empty rows
+            }
+            if (m == 0) acc[0] += sum;
+            else if (m == 1) acc[1] += sum;
+            else acc[2] += sum;
+            e = base + stop;
+        }
+    }
+    grid_sum<F, 3>(acc, a.partial, a.counter, a.result);
+}
+
 }  // namespace lurk
 
 using namespace lurk;
@@ -226,6 +289,7 @@ struct SpartanCtx : lurk_spartan_ctx {
     DevBuf work;                 // the prover's vectors, allocated by the first proof and kept: a fresh 0.6 GB per call at fib rc = 100
                                  // would cost more than the eval table saves
     size_t tnnz = 0, threads = 0;
+    uint64_t nnz[3] = {0, 0, 0};
 
     // Az, Bz, Cz, u Cz + E, eq, E padded (2^log_rows each) | z padded, its working copy, abc (2 num_vars each)
     int work_area(F **out) {
@@ -254,6 +318,7 @@ struct SpartanCtx : lurk_spartan_ctx {
             csr[m].row_ptr = rp[m].as<uint64_t>();
             csr[m].col = col[m].as<uint32_t>();
             csr[m].val = val[m].p;
+            this->nnz[m] = nnz;
             tnnz += nnz;
         }
         // merged transpose over the padded z's 2 num_vars columns
@@ -301,6 +366,37 @@ struct SpartanCtx : lurk_spartan_ctx {
         a.slot_first = slots.as<F>() + threads;
         a.ticket = ticket.as<unsigned>();
         sp_eval_table_kernel<F><<<(unsigned)grid, 256, 0, s>>>(a);
+        LURK_CUDA_TRY(cudaGetLastError());
+        return LURK_OK;
+    }
+
+    // (A, B, C)(rx, ry) into res[0..3) of the scratch's pinned result slots, Montgomery; asynchronous on s.  rx: log_rows elements,
+    // ry: log_vars + 1.
+    int matrix_evals(const F *rx, const F *ry, ScScratch<F> &sc, F *res, cudaStream_t s) {
+        SpMatArgs<F> a;
+        memset(&a, 0, sizeof a);
+        for (int m = 0; m < 3; m++) {
+            a.rp[m] = csr[m].row_ptr;
+            a.col[m] = csr[m].col;
+            a.val[m] = static_cast<const F *>(csr[m].val);
+            a.off[m + 1] = a.off[m] + nnz[m];
+        }
+        a.chunks = (a.off[3] + SP_CHUNK - 1) / SP_CHUNK;
+        a.rows = rows;
+        a.n_w = n_w;
+        a.num_vars = num_vars;
+        a.x.l = log_rows;
+        a.y.l = log_vars + 1;
+        for (int j = 0; j < a.x.l; j++) { a.x.hi[j] = rx[j]; a.x.lo[j] = F::one() - rx[j]; }
+        for (int j = 0; j < a.y.l; j++) { a.y.hi[j] = ry[j]; a.y.lo[j] = F::one() - ry[j]; }
+        a.partial = sc.partial;
+        a.counter = sc.counter;
+        a.result = res;
+        const size_t smem = (size_t)(tensor_groups(a.x.l) + tensor_groups(a.y.l)) * TENSOR_GROUP * sizeof(F);
+        LURK_CUDA_TRY(cudaFuncSetAttribute(sp_matrix_eval_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const uint64_t want = (a.chunks + 255) / 256;
+        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(want, 2 * (uint64_t)sm_count()));
+        sp_matrix_eval_kernel<F><<<grid, 256, smem, s>>>(a);
         LURK_CUDA_TRY(cudaGetLastError());
         return LURK_OK;
     }
@@ -468,6 +564,222 @@ static int spartan_prove(int n, lurk_spartan_ctx *const *ctxs, const void *const
     return LURK_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ the verifier
+template <class F>
+static F pow2(int k) { F r = F::one(); const F two = F::from_u64(2); for (int j = 0; j < k; j++) r = r * two; return r; }
+
+// eq(a, b) = prod_j (a_j b_j + (1 - a_j)(1 - b_j))
+template <class F>
+static F eq_at(const F *a, const F *b, int l) {
+    F r = F::one();
+    for (int j = 0; j < l; j++) r = r * (a[j] * b[j] + (F::one() - a[j]) * (F::one() - b[j]));
+    return r;
+}
+
+// The MLE of (tail | 0 ..) of 2^l elements at y[0 .. l): with 2^q >= |tail| the top l - q variables only select the zero-padded prefix.
+template <class F>
+static F tail_eval(std::vector<F> v, const F *y, int l) {
+    int q = 0;
+    while (((size_t)1 << q) < v.size()) q++;
+    F scale = F::one();
+    for (int j = 0; j < l - q; j++) scale = scale * (F::one() - y[j]);
+    v.resize((size_t)1 << q, F::zero());
+    for (int j = l - q; j < l; j++) {
+        const size_t half = v.size() / 2;
+        for (size_t i = 0; i < half; i++) v[i] = v[i] + y[j] * (v[i + half] - v[i]);
+        v.resize(half);
+    }
+    return scale * v[0];
+}
+
+static bool all_reduced(const uint8_t *in, size_t count, int fmt, int field_id) {
+    return dispatch_field(field_id, [&](auto f) {
+        using F = decltype(f);
+        F x;
+        for (size_t i = 0; i < count; i++)
+            if (!fe_in(in + 32 * i, fmt, x)) return 0;
+        return 1;
+    }) == 1;
+}
+
+// Round j of a sum-check of degree `deg` as the proof holds it: s(0) | .. | s(deg) (LURK_SPARTAN_ROUNDS_EVALS; the round must sum to the
+// running claim) or Arecibo's CompressedUniPoly, every coefficient but the linear one, constant first (LURK_SPARTAN_ROUNDS_COMPRESSED;
+// decompress(hint): the linear coefficient is what makes s(0) + s(1) the claim).  Each round hands s(0) | .. | s(deg) to the transcript
+// (phase, round first_round + j) and continues from s(r_j).  Returns LURK_OK with ok = false when a round does not sum to its claim.
+template <class F>
+static int sumcheck_verify(const uint8_t *rounds_in, int rounds, int deg, int rounds_fmt, lurk_spartan_challenge_fn fn, void *user, int phase,
+                           int first_round, int fmt, F &claim, std::vector<F> &r, bool &ok) {
+    const ScLagrange<F> lagrange(deg + 1);
+    const int per = rounds_fmt == LURK_SPARTAN_ROUNDS_EVALS ? deg + 1 : deg;
+    r.assign(rounds, F::zero());
+    ok = true;
+    for (int j = 0; j < rounds; j++) {
+        const uint8_t *in = rounds_in + (size_t)32 * per * j;
+        F ev[4];
+        if (rounds_fmt == LURK_SPARTAN_ROUNDS_EVALS) {
+            for (int t = 0; t <= deg; t++) fe_in(in + 32 * t, fmt, ev[t]);
+            if (ev[0] + ev[1] != claim) { ok = false; return LURK_OK; }
+        } else {
+            F c[4];
+            fe_in(in, fmt, c[0]);
+            c[1] = claim - c[0] - c[0];
+            for (int t = 2; t <= deg; t++) { fe_in(in + 32 * (t - 1), fmt, c[t]); c[1] = c[1] - c[t]; }
+            for (int x = 0; x <= deg; x++) {
+                const F xv = F::from_u64((uint64_t)x);
+                F v = c[deg];
+                for (int t = deg - 1; t >= 0; t--) v = v * xv + c[t];
+                ev[x] = v;
+            }
+        }
+        uint8_t msg[4 * 32];
+        for (int t = 0; t <= deg; t++) fe_out(ev[t], fmt, msg + 32 * t);
+        LURK_TRY(ask(fn, user, phase, first_round + j, msg, (size_t)32 * (deg + 1), fmt, r[j]));
+        claim = lagrange.eval(ev, r[j]);
+    }
+    return LURK_OK;
+}
+
+// RelaxedR1CSSNARK::verify (batched = false, n = 1) or BatchedRelaxedR1CSSNARK::verify up to the opening, then the verifier of
+// batch_eval_reduce over [W_i .., E_i ..]: the same transcript calls as spartan_prove, in the same order.  The matrices' evaluations at
+// (rx_i, ry_i) are one sp_matrix_eval_kernel launch per instance and one synchronisation; everything else is O(log) host arithmetic (and
+// O(n_x) for eval_X).  A failed check returns LURK_OK with *accepted = 0.
+template <class F>
+static int spartan_verify(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u_in, const uint8_t *const *X_in, lurk_spartan_proof *proof,
+                          int rounds_fmt, lurk_spartan_challenge_fn fn, void *user, int *accepted, int fmt, cudaStream_t s, bool batched) {
+    *accepted = 0;
+    std::vector<SpartanCtx<F> *> C(n);
+    std::vector<int> S(n), T(n);
+    int maxS = 0, maxT = 0;
+    for (int i = 0; i < n; i++) {
+        C[i] = static_cast<SpartanCtx<F> *>(ctxs[i]);
+        S[i] = C[i]->log_rows;
+        T[i] = C[i]->log_vars + 1;
+        maxS = std::max(maxS, S[i]);
+        maxT = std::max(maxT, T[i]);
+    }
+    const int m = std::max(maxS, maxT - 1);
+    const bool evals = rounds_fmt == LURK_SPARTAN_ROUNDS_EVALS;
+    // every input is checked before the first transcript call: a value >= p is an error, not a rejection
+    const int fid = ctxs[0]->field_id;
+    std::vector<F> u(n), cl(4 * (size_t)n), ew(n), left(2 * (size_t)n);
+    std::vector<std::vector<F>> X(n);
+    for (int i = 0; i < n; i++) {
+        if (!fe_in(u_in + 32 * i, fmt, u[i])) { set_error("u of instance %d is not reduced", i); return LURK_ERR_RANGE; }
+        X[i].resize(C[i]->n_x);
+        for (uint64_t k = 0; k < C[i]->n_x; k++)
+            if (!fe_in(X_in[i] + 32 * k, fmt, X[i][k])) { set_error("X[%llu] of instance %d is not reduced", (unsigned long long)k, i); return LURK_ERR_RANGE; }
+    }
+    struct Field { const uint8_t *p; size_t count; const char *name; F *out; };
+    const Field fields[] = {{proof->outer_rounds, (size_t)maxS * (evals ? 4 : 3), "outer_rounds", nullptr},
+                            {proof->inner_rounds, (size_t)maxT * (evals ? 3 : 2), "inner_rounds", nullptr},
+                            {proof->reduce_rounds, (size_t)m * (evals ? 3 : 2), "reduce_rounds", nullptr},
+                            {proof->claims, 4 * (size_t)n, "claims", cl.data()},
+                            {proof->eval_W, (size_t)n, "eval_W", ew.data()},
+                            {proof->claims_left, 2 * (size_t)n, "claims_left", left.data()}};
+    for (const Field &f : fields) {
+        if (!all_reduced(f.p, f.count, fmt, fid)) { set_error("proof field %s holds a value that is not reduced", f.name); return LURK_ERR_RANGE; }
+        for (size_t k = 0; f.out && k < f.count; k++) fe_in(f.p + 32 * k, fmt, f.out[k]);
+    }
+
+    // tau, outer_r
+    std::vector<std::vector<F>> tau(n);
+    F outer_r = F::one();
+    if (!batched) {
+        tau[0].resize(S[0]);
+        for (int j = 0; j < S[0]; j++) LURK_TRY(ask(fn, user, LURK_SPARTAN_TAU, j, nullptr, 0, fmt, tau[0][j]));
+    } else {
+        F t;
+        LURK_TRY(ask(fn, user, LURK_SPARTAN_TAU, 0, nullptr, 0, fmt, t));
+        for (int i = 0; i < n; i++) {
+            tau[i].resize(S[i]);
+            tau[i][0] = t;
+            for (int j = 1; j < S[i]; j++) tau[i][j] = tau[i][j - 1] * tau[i][j - 1];
+        }
+        LURK_TRY(ask(fn, user, LURK_SPARTAN_OUTER_R, 0, nullptr, 0, fmt, outer_r));
+    }
+    // outer sum-check: claim 0, final value sum_i outer_r^i eq(tau_i, rx_i) (Az Bz - u Cz - E)_i
+    bool ok = true;
+    F e = F::zero();
+    std::vector<F> rx, ry, rr;
+    LURK_TRY(sumcheck_verify<F>(proof->outer_rounds, maxS, 3, rounds_fmt, fn, user, LURK_SPARTAN_OUTER, 0, fmt, e, rx, ok));
+    if (!ok) return LURK_OK;
+    F want = F::zero(), c = F::one();
+    for (int i = 0; i < n; i++, c = c * outer_r) {
+        const F *k = &cl[4 * i];
+        want += c * eq_at(tau[i].data(), rx.data() + (maxS - S[i]), S[i]) * (k[0] * k[1] - u[i] * k[2] - k[3]);
+    }
+    if (e != want) return LURK_OK;
+    // r, the inner sum-check: claim sum_i (r^3)^i 2^(maxT - T_i) joint_i
+    F r;
+    LURK_TRY(ask(fn, user, LURK_SPARTAN_CLAIMS, 0, proof->claims, 4 * 32 * (size_t)n, fmt, r));
+    const F r2 = r * r, r3 = r2 * r;
+    e = F::zero();
+    c = F::one();
+    for (int i = 0; i < n; i++, c = c * r3) e += c * (cl[4 * i] + r * cl[4 * i + 1] + r2 * cl[4 * i + 2]) * pow2<F>(maxT - T[i]);
+    LURK_TRY(sumcheck_verify<F>(proof->inner_rounds, maxT, 2, rounds_fmt, fn, user, LURK_SPARTAN_INNER, 0, fmt, e, ry, ok));
+    if (!ok) return LURK_OK;
+    ScScratch<F> sc;
+    LURK_TRY(sc.init(s));
+    for (int i = 0; i < n; i++) LURK_TRY(C[i]->matrix_evals(rx.data() + (maxS - S[i]), ry.data() + (maxT - T[i]), sc, sc.result + 3 * i, s));
+    LURK_CUDA_TRY(cudaStreamSynchronize(s));
+    const F *abc = static_cast<const F *>(sc.pinned);
+    want = F::zero();
+    c = F::one();
+    for (int i = 0; i < n; i++, c = c * r3) {
+        const F *y = ry.data() + (maxT - T[i]);
+        std::vector<F> tail(1 + X[i].size());
+        tail[0] = u[i];
+        std::copy(X[i].begin(), X[i].end(), tail.begin() + 1);
+        const F eval_z = (F::one() - y[0]) * ew[i] + y[0] * tail_eval(std::move(tail), y + 1, T[i] - 1);
+        want += c * (abc[3 * i] + r * abc[3 * i + 1] + r2 * abc[3 * i + 2]) * eval_z;
+    }
+    if (e != want) return LURK_OK;
+
+    // batch_eval_reduce's verifier over [W_0 .. W_{n-1}, E_0 .. E_{n-1}] at [ry_i[1:] .., rx_i ..]
+    const int nc = 2 * n;
+    std::vector<int> nv(nc);
+    std::vector<const F *> pts(nc);
+    std::vector<F> ev(nc);
+    std::vector<uint8_t> msg(32 * (size_t)nc);
+    for (int i = 0; i < n; i++) {
+        nv[i] = T[i] - 1;
+        pts[i] = ry.data() + (maxT - T[i]) + 1;
+        ev[i] = ew[i];
+        nv[n + i] = S[i];
+        pts[n + i] = rx.data() + (maxS - S[i]);
+        ev[n + i] = cl[4 * i + 3];
+    }
+    for (int k = 0; k < nc; k++) fe_out(ev[k], fmt, msg.data() + 32 * k);
+    F rho;
+    LURK_TRY(ask(fn, user, LURK_SPARTAN_BATCH_EVAL, 0, msg.data(), msg.size(), fmt, rho));
+    e = F::zero();
+    c = F::one();
+    for (int k = 0; k < nc; k++, c = c * rho) e += c * ev[k] * pow2<F>(m - nv[k]);
+    LURK_TRY(sumcheck_verify<F>(proof->reduce_rounds, m, 2, rounds_fmt, fn, user, LURK_SPARTAN_BATCH_EVAL, 1, fmt, e, rr, ok));
+    if (!ok) return LURK_OK;
+    want = F::zero();
+    c = F::one();
+    for (int k = 0; k < nc; k++, c = c * rho) want += c * eq_at(pts[k], rr.data() + (m - nv[k]), nv[k]) * left[k];
+    if (e != want) return LURK_OK;
+    F gamma;
+    LURK_TRY(ask(fn, user, LURK_SPARTAN_BATCH_EVAL, m + 1, proof->claims_left, 32 * (size_t)nc, fmt, gamma));
+    std::vector<F> w(nc);
+    F joint = F::zero();
+    for (int k = 0; k < nc; k++) {
+        w[k] = k ? w[k - 1] * gamma : F::one();
+        F scale = w[k];
+        for (int j = 0; j < m - nv[k]; j++) scale = scale * (F::one() - rr[j]);
+        joint += scale * left[k];
+    }
+    *accepted = 1;
+    for (int j = 0; proof->r_x && j < maxS; j++) fe_out(rx[j], fmt, proof->r_x + 32 * j);
+    for (int j = 0; proof->r_y && j < maxT; j++) fe_out(ry[j], fmt, proof->r_y + 32 * j);
+    for (int j = 0; proof->r && j < m; j++) fe_out(rr[j], fmt, proof->r + 32 * j);
+    for (int k = 0; proof->weights && k < nc; k++) fe_out(w[k], fmt, proof->weights + 32 * k);
+    if (proof->joint_eval) fe_out(joint, fmt, proof->joint_eval);
+    return LURK_OK;
+}
+
 }  // namespace lurk
 
 static int ceil_log2(uint64_t x) { int l = 0; while (((uint64_t)1 << l) < x) l++; return l; }
@@ -500,6 +812,36 @@ static int check_prove_args(int n, lurk_spartan_ctx *const *ctxs, const void *co
     for (int i = 0; i < n; i++) {
         if (overlaps(d_joint, joint_bytes, d_z[i], 32 * ctxs[i]->z_len())) { set_error("d_joint overlaps d_z of instance %d", i); return LURK_ERR_ARG; }
         if (overlaps(d_joint, joint_bytes, d_E[i], 32 * ctxs[i]->rows)) { set_error("d_joint overlaps d_E of instance %d", i); return LURK_ERR_ARG; }
+    }
+    return LURK_OK;
+}
+
+// argument checks of both verifiers, before any device work (the contexts are only read for their sizes and field)
+static int check_verify_args(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u, const uint8_t *const *X, const lurk_spartan_proof *proof,
+                             int rounds_fmt, lurk_spartan_challenge_fn fn, const int *accepted, int fmt) {
+    if (n < 1 || n > SP_MAX_INSTANCES) { set_error("1..%d instances, got %d", SP_MAX_INSTANCES, n); return LURK_ERR_ARG; }
+    if (!ctxs || !X) { set_error("null instance array"); return LURK_ERR_ARG; }
+    if (!u) { set_error("null u"); return LURK_ERR_ARG; }
+    if (!fn) { set_error("null challenge callback"); return LURK_ERR_ARG; }
+    if (!accepted) { set_error("null accepted"); return LURK_ERR_ARG; }
+    if (!proof) { set_error("null proof record"); return LURK_ERR_ARG; }
+    if (!proof->outer_rounds || !proof->claims || !proof->inner_rounds || !proof->eval_W || !proof->reduce_rounds || !proof->claims_left) {
+        set_error("null proof field (outer_rounds, claims, inner_rounds, eval_W, reduce_rounds and claims_left are read)");
+        return LURK_ERR_ARG;
+    }
+    if (fmt != LURK_FMT_CANONICAL && fmt != LURK_FMT_MONTGOMERY) { set_error("bad format %d", fmt); return LURK_ERR_ARG; }
+    if (rounds_fmt != LURK_SPARTAN_ROUNDS_EVALS && rounds_fmt != LURK_SPARTAN_ROUNDS_COMPRESSED) { set_error("unknown rounds_fmt %d", rounds_fmt); return LURK_ERR_ARG; }
+    for (int i = 0; i < n; i++) {
+        if (!ctxs[i]) { set_error("null context %d", i); return LURK_ERR_ARG; }
+        for (int k = 0; k < i; k++)
+            if (ctxs[k] == ctxs[i]) { set_error("instances %d and %d share a context", k, i); return LURK_ERR_ARG; }
+    }
+    for (int i = 0; i < n; i++) {
+        if (ctxs[i]->field_id != ctxs[0]->field_id) {
+            set_error("context %d is over field %d, context 0 over field %d", i, ctxs[i]->field_id, ctxs[0]->field_id);
+            return LURK_ERR_ARG;
+        }
+        if (ctxs[i]->n_x && !X[i]) { set_error("null X of instance %d", i); return LURK_ERR_ARG; }
     }
     return LURK_OK;
 }
@@ -586,6 +928,49 @@ int lurk_spartan_eval_table_dev(lurk_spartan_ctx *ctx, const void *d_eq_rx, cons
         F rv;
         if (!fe_in(r, fmt, rv)) { set_error("r is not reduced"); return LURK_ERR_RANGE; }
         return static_cast<SpartanCtx<F> *>(ctx)->eval_table(static_cast<const F *>(d_eq_rx), rv, static_cast<F *>(d_out), static_cast<cudaStream_t>(stream));
+    });
+}
+
+int lurk_spartan_matrix_evals_dev(lurk_spartan_ctx *ctx, const uint8_t *r_x, const uint8_t *r_y, uint8_t out[96], int fmt, void *stream) {
+    if (!ctx || !r_x || !r_y || !out) { set_error("null argument"); return LURK_ERR_ARG; }
+    if (fmt != LURK_FMT_CANONICAL && fmt != LURK_FMT_MONTGOMERY) { set_error("bad format %d", fmt); return LURK_ERR_ARG; }
+    LURK_TRY(require_gpu());
+    return dispatch_field(ctx->field_id, [&](auto f) {
+        using F = decltype(f);
+        SpartanCtx<F> *c = static_cast<SpartanCtx<F> *>(ctx);
+        std::vector<F> x(c->log_rows), y(c->log_vars + 1);
+        for (int j = 0; j < c->log_rows; j++)
+            if (!fe_in(r_x + 32 * j, fmt, x[j])) { set_error("r_x[%d] is not reduced", j); return LURK_ERR_RANGE; }
+        for (int j = 0; j <= c->log_vars; j++)
+            if (!fe_in(r_y + 32 * j, fmt, y[j])) { set_error("r_y[%d] is not reduced", j); return LURK_ERR_RANGE; }
+        const cudaStream_t s = static_cast<cudaStream_t>(stream);
+        ScScratch<F> sc;
+        LURK_TRY(sc.init(s));
+        LURK_TRY(c->matrix_evals(x.data(), y.data(), sc, sc.result, s));
+        F res[3];
+        LURK_TRY(sc.fetch(3, res, s));
+        for (int k = 0; k < 3; k++) fe_out(res[k], fmt, out + 32 * k);
+        return LURK_OK;
+    });
+}
+
+int lurk_spartan_verify(lurk_spartan_ctx *ctx, const uint8_t u[32], const uint8_t *X, lurk_spartan_proof *proof, int rounds_fmt,
+                        lurk_spartan_challenge_fn challenge, void *user, int *accepted, int fmt, void *stream) {
+    if (!ctx) { set_error("null context"); return LURK_ERR_ARG; }
+    const uint8_t *const xs[1] = {X};
+    LURK_TRY(check_verify_args(1, &ctx, u, xs, proof, rounds_fmt, challenge, accepted, fmt));
+    LURK_TRY(require_gpu());
+    return dispatch_field(ctx->field_id, [&](auto f) {
+        return spartan_verify<decltype(f)>(1, &ctx, u, xs, proof, rounds_fmt, challenge, user, accepted, fmt, static_cast<cudaStream_t>(stream), false);
+    });
+}
+
+int lurk_spartan_verify_batch(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u, const uint8_t *const *X, lurk_spartan_proof *proof,
+                              int rounds_fmt, lurk_spartan_challenge_fn challenge, void *user, int *accepted, int fmt, void *stream) {
+    LURK_TRY(check_verify_args(n, ctxs, u, X, proof, rounds_fmt, challenge, accepted, fmt));
+    LURK_TRY(require_gpu());
+    return dispatch_field(ctxs[0]->field_id, [&](auto f) {
+        return spartan_verify<decltype(f)>(n, ctxs, u, X, proof, rounds_fmt, challenge, user, accepted, fmt, static_cast<cudaStream_t>(stream), true);
     });
 }
 

@@ -243,14 +243,6 @@ static int shifted_challenge(void *user, int round, const uint8_t *message, size
     return c->fn(c->user, round + 1, message, message_len, challenge_out);
 }
 
-// stream-ordered scratch, freed (in stream order) when the call returns
-struct StreamBuf {
-    void *p = nullptr;
-    cudaStream_t s = nullptr;
-    ~StreamBuf() { if (p) cudaFreeAsync(p, s); }
-    int alloc(size_t bytes, cudaStream_t st) { s = st; LURK_CUDA_TRY(cudaMallocAsync(&p, bytes ? bytes : 16, st)); return LURK_OK; }
-};
-
 // Arecibo's batch_eval_reduce (spartan/mod.rs in the public crate, not under the reference checkout; restated): claims P_i(x_i) = e_i
 // -> rho; the batched quadratic sum-check of sum_i rho^i sum_y P_i(y) eq(x_i, y), instance i joining in round m - n_i, gives r and the
 // L_i = P_i(r[m - n_i:]); -> gamma.  PolyEvalInstance / PolyEvalWitness::batch_diff_size then treat P_i as zero-padded at the top to

@@ -135,6 +135,37 @@ def ipa_prove(curve_id, ck, ck_c, d_a_ptr, d_b_ptr, log_n, challenge, stream=0):
     return pts(Ls), pts(Rs), int.from_bytes(af.tobytes(), "little"), int.from_bytes(bf.tobytes(), "little")
 
 
+def _fes(vals):
+    return np.frombuffer(b"".join(int(v).to_bytes(32, "little") for v in vals) or bytes(32), dtype=np.uint8).copy()
+
+
+def _point_bytes(P):
+    """(x, y) or None (the identity) -> x | y | z, 96 bytes canonical"""
+    return _fes([0, 0, 0]) if P is None else _fes([P[0], P[1], 1])
+
+
+def ipa_verify(curve_id, ck, ck_c, comm, c, d_b_ptr, log_n, Ls, Rs, a_final, challenge, stream=0):
+    """InnerProductArgument::verify of <a, b> = c with comm = commit(a), from ipa_prove's transcript under the key of CommitmentKey `ck` (not
+    consumed).  ck_c: (x, y); comm, Ls, Rs: (x, y) tuples or None; d_b_ptr: 2^log_n Montgomery elements on the device (not modified);
+    challenge(round, L | R bytes) -> int as for ipa_prove.  Returns (accepted, ck_hat point or None, b_hat)."""
+    assert len(Ls) == log_n and len(Rs) == log_n
+    gc = _fes([ck_c[0], ck_c[1]])
+    Lb = np.concatenate([_point_bytes(P) for P in Ls]) if log_n else np.zeros(96, dtype=np.uint8)
+    Rb = np.concatenate([_point_bytes(P) for P in Rs]) if log_n else np.zeros(96, dtype=np.uint8)
+    hat, bh = np.zeros(96, dtype=np.uint8), np.zeros(32, dtype=np.uint8)
+    acc = C.c_int(-1)
+    errors = []
+    cb = _callback(challenge, errors)
+    rc = _capi.lib().lurk_ipa_verify_dev(curve_id, ck._ctx, _capi.np_ptr(gc), _capi.np_ptr(_point_bytes(comm)), _capi.np_ptr(_fe(c)), C.c_void_p(d_b_ptr),
+                                         log_n, _capi.np_ptr(Lb), _capi.np_ptr(Rb), _capi.np_ptr(_fe(a_final)), cb, None, C.byref(acc), _capi.np_ptr(hat),
+                                         _capi.np_ptr(bh), _capi.FMT_CANONICAL, C.c_void_p(stream))
+    if errors:
+        raise errors[0]
+    _capi.check(rc)
+    h = _ints(hat)
+    return bool(acc.value), ((h[0], h[1]) if h[2] else None), int.from_bytes(bh.tobytes(), "little")
+
+
 def hyperkzg_prove(curve_id, ck, d_poly_ptr, point, challenge, stream=0):
     """provider::hyperkzg::EvaluationEngine::prove.  ck: a CommitmentKey on the KZG key; point: ints.  challenge(round, message) -> int
     with round 0 = commitments, 1 = evaluations, 2 = witness commitments.  Returns (com points, v [3][l] ints, w points)."""
@@ -513,11 +544,79 @@ class SpartanContext:
         _capi.check(_capi.lib().lurk_spartan_eval_table_dev(self._ctx, C.c_void_p(d_eq_ptr), _capi.np_ptr(_fe(r)), C.c_void_p(d_out_ptr),
                                                             _capi.FMT_CANONICAL, C.c_void_p(stream)))
 
+    def matrix_evals(self, rx, ry, stream=0):
+        """(A(rx, ry), B(rx, ry), C(rx, ry)): rx of log_rows ints, ry of log_vars + 1 ints over the padded z"""
+        assert len(rx) == self.log_rows and len(ry) == self.log_vars + 1
+        out = np.zeros(96, dtype=np.uint8)
+        _capi.check(_capi.lib().lurk_spartan_matrix_evals_dev(self._ctx, _capi.np_ptr(_fes(rx)), _capi.np_ptr(_fes(ry)), _capi.np_ptr(out),
+                                                              _capi.FMT_CANONICAL, C.c_void_p(stream)))
+        return tuple(_ints(out))
+
+    def verify(self, proof, u, X, challenge, compressed=False, stream=0):
+        """RelaxedR1CSSNARK::verify + batch_eval_reduce's verifier through lurk_spartan_verify.  proof: what prove returns (round polynomials as
+        evaluations), or with compressed=True every round as its coefficients without the linear one.  Returns (accepted, derived) with derived =
+        dict(rx, ry, r, weights, joint_eval) of an accepted proof, else None."""
+        return _spartan_verify([self], [(u, X)], proof, challenge, compressed, stream, batched=False)
+
 
 def spartan_prove_batch(ctxs, instances, challenge, d_joint_ptr=None, stream=0):
     """BatchedRelaxedR1CSSNARK::prove through lurk_spartan_prove_batch_dev.  ctxs: SpartanContext per circuit, instances: [(d_z_ptr, d_E_ptr)].
     Returns what BatchedRelaxedR1CSProver.prove returns (without E_padded)."""
     return _spartan_prove(ctxs, instances, challenge, d_joint_ptr, stream, batched=True)
+
+
+def spartan_verify_batch(ctxs, insts, proof, challenge, compressed=False, stream=0):
+    """BatchedRelaxedR1CSSNARK::verify through lurk_spartan_verify_batch.  insts: [(u, X)] per context; proof as spartan_prove_batch returns
+    it.  Returns (accepted, derived) as SpartanContext.verify."""
+    return _spartan_verify(ctxs, insts, proof, challenge, compressed, stream, batched=True)
+
+
+def _spartan_verify(ctxs, insts, proof, challenge, compressed, stream, batched):
+    n, p = len(ctxs), ctxs[0].p
+    S = [c.log_rows for c in ctxs]
+    T = [c.log_vars + 1 for c in ctxs]
+    mS, mT = max(S), max(T)
+    m = max(mS, mT - 1)
+    claims = proof["claims"] if batched else [proof["claims"]]
+    eval_W = proof["eval_W"] if batched else [proof["eval_W"]]
+    per = 0 if compressed else 1                  # a compressed round drops the linear coefficient
+    shapes = (("outer_rounds", mS, 3 + per), ("inner_rounds", mT, 2 + per), ("reduce_rounds", m, 2 + per))
+    for key, rounds, width in shapes:
+        if len(proof[key]) != rounds or any(len(rnd) != width for rnd in proof[key]):
+            raise ValueError(f"{key}: {rounds} rounds of {width} values expected")
+    if len(claims) != n or any(len(c) != 4 for c in claims) or len(eval_W) != n or len(proof["claims_left"]) != 2 * n:
+        raise ValueError("claims, eval_W or claims_left of the wrong length")
+    bufs = {key: _fes(x for rnd in proof[key] for x in rnd) for key, _, _ in shapes}
+    bufs.update(claims=_fes(x for c in claims for x in c), eval_W=_fes(eval_W), claims_left=_fes(proof["claims_left"]))
+    bufs.update({k: np.zeros(max(1, v) * 32, dtype=np.uint8) for k, v in dict(r_x=mS, r_y=mT, r=m, weights=2 * n, joint_eval=1).items()})
+    rec = _capi.SpartanProof(**{k: b.ctypes.data for k, b in bufs.items()})
+    us = _fes([u for u, _ in insts])
+    xs = [_fes(X) for _, X in insts]
+    acc = C.c_int(-1)
+    errors = []
+    cb = _spartan_callback(challenge, p, n, batched, errors)
+    fmt_r = _capi.SPARTAN_ROUNDS_COMPRESSED if compressed else _capi.SPARTAN_ROUNDS_EVALS
+    lib = _capi.lib()
+    if batched:
+        cs = (C.c_void_p * n)(*[c._ctx for c in ctxs])
+        xp = (C.c_void_p * n)(*[x.ctypes.data for x in xs])
+        rc = lib.lurk_spartan_verify_batch(n, cs, _capi.np_ptr(us), xp, C.byref(rec), fmt_r, cb, None, C.byref(acc), _capi.FMT_CANONICAL, C.c_void_p(stream))
+    else:
+        rc = lib.lurk_spartan_verify(ctxs[0]._ctx, _capi.np_ptr(us), _capi.np_ptr(xs[0]), C.byref(rec), fmt_r, cb, None, C.byref(acc), _capi.FMT_CANONICAL,
+                                     C.c_void_p(stream))
+    if errors:
+        raise errors[0]
+    _capi.check(rc)
+    if not acc.value:
+        return False, None
+    v = {k: _ints(bufs[k]) for k in ("r_x", "r_y", "r", "weights", "joint_eval")}
+    r_x, r_y = v["r_x"][:mS], v["r_y"][:mT]
+    out = dict(r=v["r"][:m], weights=v["weights"][:2 * n], joint_eval=v["joint_eval"][0])
+    if batched:
+        out.update(rx=[r_x[mS - s:] for s in S], ry=[r_y[mT - t:] for t in T])
+    else:
+        out.update(rx=r_x, ry=r_y)
+    return True, out
 
 
 def _spartan_prove(ctxs, instances, challenge, d_joint_ptr, stream, batched):
