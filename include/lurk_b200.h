@@ -385,6 +385,73 @@ int lurk_spartan_verify(lurk_spartan_ctx *ctx, const uint8_t u[32], const uint8_
 int lurk_spartan_verify_batch(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u, const uint8_t *const *X, lurk_spartan_proof *proof,
                               int rounds_fmt, lurk_spartan_challenge_fn challenge, void *user, int *accepted, int fmt, void *stream);
 
+/* Compress context: CompressedSNARK::prove (Nova's `compress`, src/proof/nova.rs:341-356; SuperNova's, supernova.rs:293-317) in one call
+ * -- for the primary and the secondary circuit, RelaxedR1CSSNARK::prove (or BatchedRelaxedR1CSSNARK::prove for SuperNova's primary),
+ * batch_eval_reduce, the joint commitment sum_i weights_i C_i and the opening of the joint polynomial -- with the two circuits proved at
+ * once, each on its own library-owned host thread and CUDA stream (Arecibo's rayon::join of S1::prove and S2::prove).
+ *
+ * Before the call, as in Arecibo's CompressedSNARK::prove, the secondary's last fresh instance is folded into its running instance
+ * (NIFS::prove of l_u_secondary into r_U_secondary): one more lurk_fold_ctx_stage_a + lurk_fold_ctx_stage_b_launch + lurk_fold_ctx_collect
+ * on the secondary's fold context with that instance in the buffer (its record carries comm_T).  The call then reads the running
+ * instances straight from the fold contexts' LURK_FOLD_BUF_Z1 / LURK_FOLD_BUF_E1 buffers, and takes their commitments from the last
+ * records (running_comm_W, running_comm_E).
+ *
+ * The context borrows the Spartan contexts (n_primary of them; 1 for Nova, 1..30 for SuperNova) and, per circuit, the evaluation engine:
+ *   LURK_PCS_HYPERKZG  ck = a context on the KZG key (the primary of the BN256 / Grumpkin cycle);
+ *   LURK_PCS_IPA       ck = a context on the Pedersen key, ck_c = the inner-product base, 64 bytes affine, unscaled.
+ * It clones each key context (the clones never share MSM scratch with a fold context on the same key; the borrowed contexts must outlive
+ * the compress context), allocates on its first proof one scratch arena per circuit -- fold chain, witness polynomials, evaluation
+ * partials, MSM clones, side streams -- sized for that circuit's joint polynomial, and keeps everything until destroy.  Every size, field
+ * and curve is checked before any device work: each key holds >= joint_len bases, the secondary's field is the primary's cycle partner,
+ * each key's scalar field is its circuit's field, and no Spartan context is passed twice. */
+#define LURK_PCS_HYPERKZG 0
+#define LURK_PCS_IPA 1
+typedef struct lurk_compress_pcs {
+    int kind;              /* LURK_PCS_* */
+    lurk_msm_ctx *ck;      /* borrowed; curve = the one whose scalar field is the circuit's field */
+    const uint8_t *ck_c;   /* IPA: 64 bytes affine in the create call's `fmt` (copied); HyperKZG: NULL */
+} lurk_compress_pcs;
+typedef struct lurk_compress_ctx lurk_compress_ctx;
+int lurk_compress_ctx_create(int n_primary, lurk_spartan_ctx *const *primary, lurk_spartan_ctx *secondary, const lurk_compress_pcs *pcs_primary,
+                             const lurk_compress_pcs *pcs_secondary, int fmt, lurk_compress_ctx **out);
+void lurk_compress_ctx_destroy(lurk_compress_ctx *ctx);
+/* device bytes the context holds (its arenas; 0 before the first proof) and the joint-polynomial lengths; any output may be NULL */
+int lurk_compress_ctx_info(lurk_compress_ctx *ctx, size_t *device_bytes, size_t *joint_len_primary, size_t *joint_len_secondary);
+/* The transcript: circuit 0 = primary, 1 = secondary; phase and round as lurk_spartan_challenge_fn, plus the opening's phase
+ * LURK_SPARTAN_PCS:
+ *   HyperKZG  rounds 0, 1, 2: the messages lurk_hyperkzg_prove_dev passes (com; v; w -- the last challenge is ignored)
+ *   IPA       round 0: comm | joint_eval (96 + 32 bytes) -> r, the scale of ck_c (InnerProductInstance absorbs comm and c, not b);
+ *             rounds 1 .. m: L | R of the inner-product argument's rounds 0 .. m - 1
+ * For one circuit the callback is called in protocol order and never concurrently with itself; the two circuits' calls may be concurrent
+ * (with LURK_COMPRESS_SEQUENTIAL they are not).  The caller absorbs each circuit's verifier-key digest and instance U into that circuit's
+ * transcript before the call, as the Spartan context requires.  Returns 0, or non-zero to abort the proof. */
+#define LURK_SPARTAN_PCS 6
+typedef int (*lurk_compress_challenge_fn)(void *user, int circuit, int phase, int round, const uint8_t *message, size_t message_len,
+                                          uint8_t challenge_out[32]);
+/* One circuit's proof, every buffer caller-owned and optional (NULL = not wanted), `fmt`.  m = log2 of the circuit's joint_len. */
+typedef struct lurk_compress_circuit_proof {
+    lurk_spartan_proof snark;  /* as lurk_spartan_prove_dev / _batch_dev write it */
+    uint8_t *comm;             /* 96: the joint commitment sum_i weights_i C_i over [comm_W_0 .., comm_E_0 ..] */
+    uint8_t *com;              /* HyperKZG: (m - 1) x 96 */
+    uint8_t *w;                /* HyperKZG: 3 x 96 */
+    uint8_t *v;                /* HyperKZG: 3 x m x 32 */
+    uint8_t *L, *R;            /* IPA: m x 96 each */
+    uint8_t *a_final, *b_final;   /* IPA: 32 each */
+} lurk_compress_circuit_proof;
+typedef struct lurk_compress_proof {
+    lurk_compress_circuit_proof primary, secondary;
+} lurk_compress_proof;
+#define LURK_COMPRESS_SEQUENTIAL 1  /* the secondary proof after the primary one, on the same host thread */
+#define LURK_COMPRESS_BATCHED 2     /* the primary is BatchedRelaxedR1CSSNARK (SuperNova), also with n_primary = 1 */
+/* d_z[i] / d_E[i]: primary instance i on the device, laid out as LURK_FOLD_BUF_Z1 / LURK_FOLD_BUF_E1 hold it (read, never written);
+ * comm_W[i] / comm_E[i]: its commitments (96 bytes, `fmt`); d_z2, d_E2, comm_W2, comm_E2: the secondary's.  n_primary must be the
+ * number of primary contexts.  The primary proof runs on `stream`, the secondary on the context's worker stream (after the work queued
+ * on `stream` so far); both host threads are joined before the call returns, errors included.  A failed callback or any other error
+ * returns its code with a message naming the circuit; the context stays usable.  One call at a time per context. */
+int lurk_compress_prove_dev(lurk_compress_ctx *ctx, int n_primary, const void *const *d_z, const void *const *d_E, const uint8_t *const *comm_W,
+                            const uint8_t *const *comm_E, const void *d_z2, const void *d_E2, const uint8_t comm_W2[96], const uint8_t comm_E2[96],
+                            lurk_compress_challenge_fn challenge, void *user, int flags, lurk_compress_proof *out, int fmt, void *stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * S5  Fold helpers on device-resident vectors (Arecibo NIFS::prove / R1CSShape::commit_T /
  *     RelaxedR1CSWitness::fold; SURVEY.md Appendix B).  All vectors Montgomery form on the device.

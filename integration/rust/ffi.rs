@@ -38,6 +38,28 @@ pub const LURK_SPARTAN_OUTER: c_int = 2;
 pub const LURK_SPARTAN_CLAIMS: c_int = 3;
 pub const LURK_SPARTAN_INNER: c_int = 4;
 pub const LURK_SPARTAN_BATCH_EVAL: c_int = 5;
+pub const LURK_SPARTAN_PCS: c_int = 6;
+#[repr(C)]
+pub struct lurk_compress_ctx { _private: [u8; 0] }
+pub const LURK_PCS_HYPERKZG: c_int = 0;
+pub const LURK_PCS_IPA: c_int = 1;
+pub const LURK_COMPRESS_SEQUENTIAL: c_int = 1;
+pub const LURK_COMPRESS_BATCHED: c_int = 2;
+/// one circuit's evaluation engine (include/lurk_b200.h: lurk_compress_pcs); ck_c: IPA's 64-byte affine base, null for HyperKZG
+#[repr(C)]
+pub struct lurk_compress_pcs { pub kind: c_int, pub ck: *mut lurk_msm_ctx, pub ck_c: *const u8 }
+/// one circuit's CompressedSNARK half: the Spartan proof, the joint commitment and the opening (HyperKZG: com, w, v; IPA: L, R, a/b_final)
+#[repr(C)]
+pub struct lurk_compress_circuit_proof {
+    pub snark: lurk_spartan_proof, pub comm: *mut u8, pub com: *mut u8, pub w: *mut u8, pub v: *mut u8, pub l: *mut u8, pub r: *mut u8,
+    pub a_final: *mut u8, pub b_final: *mut u8,
+}
+#[repr(C)]
+pub struct lurk_compress_proof { pub primary: lurk_compress_circuit_proof, pub secondary: lurk_compress_circuit_proof }
+/// `int (*)(void *user, int circuit, int phase, int round, const uint8_t *message, size_t message_len, uint8_t challenge_out[32])`: circuit 0 =
+/// primary, 1 = secondary; the two circuits' calls may come from two threads at once (one transcript per circuit).
+pub type lurk_compress_challenge_fn = unsafe extern "C" fn(user: *mut c_void, circuit: c_int, phase: c_int, round: c_int, message: *const u8,
+                                                           message_len: usize, challenge_out: *mut u8) -> c_int;
 #[repr(C)]
 #[derive(Clone, Copy)]
 pub struct lurk_dag_node { pub kind: u8, pub reserved: u8, pub tag: [u16; 4], pub child: [u32; 4] }
@@ -133,6 +155,18 @@ extern "C" {
     pub fn lurk_ipa_verify_dev(curve_id: c_int, ck: *mut lurk_msm_ctx, ck_c: *const u8, comm: *const u8, c: *const u8, d_b: *const c_void, log_n: c_int,
                                l: *const u8, r: *const u8, a_final: *const u8, challenge: lurk_challenge_fn, user: *mut c_void, accepted: *mut c_int,
                                ck_hat_out: *mut u8, b_hat_out: *mut u8, fmt: c_int, stream: *mut c_void) -> c_int;
+    // CompressedSNARK::prove in one call.  Before it, fold l_u_secondary into r_U_secondary (Arecibo's NIFS::prove) with one more
+    // lurk_fold_ctx_stage_a + lurk_fold_ctx_stage_b_launch + lurk_fold_ctx_collect on the secondary fold context; then pass both fold
+    // contexts' LURK_FOLD_BUF_Z1 / _E1 pointers and the records' running commitments.
+    pub fn lurk_compress_ctx_create(n_primary: c_int, primary: *const *mut lurk_spartan_ctx, secondary: *mut lurk_spartan_ctx,
+                                    pcs_primary: *const lurk_compress_pcs, pcs_secondary: *const lurk_compress_pcs, fmt: c_int,
+                                    out: *mut *mut lurk_compress_ctx) -> c_int;
+    pub fn lurk_compress_ctx_destroy(ctx: *mut lurk_compress_ctx);
+    pub fn lurk_compress_ctx_info(ctx: *mut lurk_compress_ctx, device_bytes: *mut usize, joint_len_primary: *mut usize, joint_len_secondary: *mut usize) -> c_int;
+    pub fn lurk_compress_prove_dev(ctx: *mut lurk_compress_ctx, n_primary: c_int, d_z: *const *const c_void, d_e: *const *const c_void,
+                                   comm_w: *const *const u8, comm_e: *const *const u8, d_z2: *const c_void, d_e2: *const c_void, comm_w2: *const u8,
+                                   comm_e2: *const u8, challenge: lurk_compress_challenge_fn, user: *mut c_void, flags: c_int,
+                                   out: *mut lurk_compress_proof, fmt: c_int, stream: *mut c_void) -> c_int;
 }
 pub const LURK_SPARTAN_ROUNDS_EVALS: c_int = 0;
 pub const LURK_SPARTAN_ROUNDS_COMPRESSED: c_int = 1;

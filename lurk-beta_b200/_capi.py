@@ -61,6 +61,26 @@ class SpartanProof(C.Structure):
                                                  "claims_left", "weights", "joint_eval")]
 
 
+# the compress context (lurk_compress_*)
+PCS_HYPERKZG, PCS_IPA = 0, 1
+SPARTAN_PCS = 6
+COMPRESS_SEQUENTIAL, COMPRESS_BATCHED = 1, 2
+# lurk_compress_challenge_fn: int (*)(void *user, int circuit, int phase, int round, const uint8_t *message, size_t message_len, uint8_t out[32])
+COMPRESS_CHALLENGE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint8), C.c_size_t, C.POINTER(C.c_uint8))
+
+
+class CompressPcs(C.Structure):
+    _fields_ = [("kind", C.c_int), ("ck", C.c_void_p), ("ck_c", C.c_void_p)]
+
+
+class CompressCircuitProof(C.Structure):
+    _fields_ = [("snark", SpartanProof)] + [(name, C.c_void_p) for name in ("comm", "com", "w", "v", "L", "R", "a_final", "b_final")]
+
+
+class CompressProof(C.Structure):
+    _fields_ = [("primary", CompressCircuitProof), ("secondary", CompressCircuitProof)]
+
+
 # every symbol declared in include/lurk_b200.h: name -> (restype, argtypes)
 PROTOTYPES = {
     "lurk_last_error": (C.c_char_p, []),
@@ -124,6 +144,11 @@ PROTOTYPES = {
     "lurk_spartan_verify": (_i, [_vp, _vp, _vp, C.POINTER(SpartanProof), _i, SPARTAN_CHALLENGE_FN, _vp, C.POINTER(_i), _i, _vp]),
     "lurk_spartan_verify_batch": (_i, [_i, C.POINTER(_vp), _vp, C.POINTER(_vp), C.POINTER(SpartanProof), _i, SPARTAN_CHALLENGE_FN, _vp, C.POINTER(_i),
                                        _i, _vp]),
+    "lurk_compress_ctx_create": (_i, [_i, C.POINTER(_vp), _vp, C.POINTER(CompressPcs), C.POINTER(CompressPcs), _i, C.POINTER(_vp)]),
+    "lurk_compress_ctx_destroy": (None, [_vp]),
+    "lurk_compress_ctx_info": (_i, [_vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
+    "lurk_compress_prove_dev": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _vp, _vp, _vp, _vp, COMPRESS_CHALLENGE_FN, _vp, _i,
+                                     C.POINTER(CompressProof), _i, _vp]),
     "lurk_ipa_verify_dev": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, CHALLENGE_FN, _vp, C.POINTER(_i), _vp, _vp, _i, _vp]),
     "lurk_axpy_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lurk_spmv_csr_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),

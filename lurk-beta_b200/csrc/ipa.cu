@@ -7,6 +7,7 @@
 #include "common.cuh"
 #include "sumcheck.cuh"
 #include "sc_scratch.cuh"
+#include "pcs.cuh"
 #include "tensor.cuh"
 
 #include <algorithm>
@@ -110,8 +111,9 @@ __global__ void __launch_bounds__(256) fill_one_kernel(F *w, size_t n) {
     for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += (size_t)gridDim.x * blockDim.x) store_fe(w + idx, one);
 }
 
+// The key weights, the clone, the side stream and the event come from the arena A, grown where the one-shot entry point allocated them.
 template <class C>
-static int ipa_prove(lurk_msm_ctx *ck, const uint8_t *gc_bytes, void *d_a, void *d_b, int log_n, lurk_challenge_fn challenge, void *user,
+static int ipa_prove(lurk_msm_ctx *ck, PcsArena &A, const uint8_t *gc_bytes, void *d_a, void *d_b, int log_n, lurk_challenge_fn challenge, void *user,
                      uint8_t *L_out, uint8_t *R_out, uint8_t *a_final, uint8_t *b_final, int fmt, cudaStream_t s) {
     using Fb = typename C::Base;
     using Fs = typename C::Scalar;
@@ -122,18 +124,16 @@ static int ipa_prove(lurk_msm_ctx *ck, const uint8_t *gc_bytes, void *d_a, void 
     LURK_TRY(sc.init(s));
     Fs *a = static_cast<Fs *>(d_a), *b = static_cast<Fs *>(d_b);
     const size_t n = (size_t)1 << log_n;
-    DevBuf wbuf;
-    LURK_TRY(wbuf.alloc(3 * n * sizeof(Fs)));
-    Fs *W = wbuf.as<Fs>(), *sl = W + n, *sr = W + 2 * n;
+    LURK_TRY(PcsArena::grow(A.weights, 3 * n * sizeof(Fs)));
+    Fs *W = A.weights.as<Fs>(), *sl = W + n, *sr = W + 2 * n;
     fill_one_kernel<Fs><<<sc_grid(n, 256), 256, 0, s>>>(W, n);
     LURK_CUDA_TRY(cudaGetLastError());
     // L and R of a round are independent: the second one runs on a clone of the context (same resident key, own scratch) and a side stream
-    MsmCloneGuard ck_r;
-    LURK_TRY(lurk_msm_ctx_clone(ck, &ck_r.c));
-    StreamGuard s_r;
-    LURK_TRY(s_r.create());
-    EventGuard weighted;
-    LURK_TRY(weighted.create());
+    LURK_TRY(A.clones(ck, 1));
+    MsmCloneGuard &ck_r = A.clone[0];
+    StreamGuard &s_r = A.side[0];
+    LURK_TRY(A.event());
+    EventGuard &weighted = A.ready;
     size_t m = n;
     for (int round = 0; round < log_n; round++) {
         const size_t half = m / 2;
@@ -361,6 +361,78 @@ static int ipa_verify(lurk_msm_ctx *ck, const uint8_t *gc_bytes, const uint8_t *
     return LURK_OK;
 }
 
+int ipa_prove_arena(int curve_id, lurk_msm_ctx *ck, PcsArena &a, const uint8_t *gc_bytes, void *d_a, void *d_b, int log_n, lurk_challenge_fn challenge,
+                    void *user, uint8_t *L_out, uint8_t *R_out, uint8_t *a_final, uint8_t *b_final, int fmt, cudaStream_t s) {
+    return dispatch_curve(curve_id, [&](auto c) {
+        return ipa_prove<decltype(c)>(ck, a, gc_bytes, d_a, d_b, log_n, challenge, user, L_out, R_out, a_final, b_final, fmt, s);
+    });
+}
+
+template <class C>
+static typename C::Base curve_b() {
+    const Affine<typename C::Base> g = curve_generator<C>();
+    return g.y.sqr() - g.x.sqr() * g.x;
+}
+
+bool points_valid(int curve_id, const uint8_t *const *points, int count, int fmt) {
+    return dispatch_curve(curve_id, [&](auto c) {
+        using C = decltype(c);
+        const typename C::Base b = curve_b<C>();
+        XYZZ<typename C::Base> p;
+        for (int k = 0; k < count; k++)
+            if (!points[k] || !point_in(points[k], fmt, b, p)) return 0;
+        return 1;
+    }) == 1;
+}
+
+// x | y -> x | y | z of the header's form
+template <class Fb>
+static void affine_to_96(const uint8_t *xy, int fmt, uint8_t out[96]) {
+    memset(out, 0, 96);
+    memcpy(out, xy, 64);
+    bool identity = true;
+    for (int i = 0; i < 64; i++) identity &= xy[i] == 0;
+    if (!identity) fe_out(Fb::one(), fmt, out + 64);
+}
+
+bool affine_valid(int curve_id, const uint8_t *xy, int fmt) {
+    return dispatch_curve(curve_id, [&](auto c) {
+        using C = decltype(c);
+        uint8_t p96[96];
+        affine_to_96<typename C::Base>(xy, fmt, p96);
+        XYZZ<typename C::Base> p;
+        return point_in(p96, fmt, curve_b<C>(), p) ? 1 : 0;
+    }) == 1;
+}
+
+int point_combination(int curve_id, const uint8_t *const *points, const uint8_t *scalars, int count, int fmt, uint8_t out[96]) {
+    return dispatch_curve(curve_id, [&](auto c) {
+        using C = decltype(c);
+        using Fb = typename C::Base;
+        using Fs = typename C::Scalar;
+        const Fb b = curve_b<C>();
+        std::vector<XYZZ<Fb>> pts(count);
+        std::vector<Fs> sc(count);
+        for (int k = 0; k < count; k++) {
+            if (!point_in(points[k], fmt, b, pts[k])) { set_error("point %d is not a point of the header's form on the curve", k); return LURK_ERR_RANGE; }
+            if (!fe_in(scalars + 32 * (size_t)k, fmt, sc[k])) { set_error("scalar %d is not reduced", k); return LURK_ERR_RANGE; }
+        }
+        point_to_bytes_fmt(host_msm(pts, sc), fmt, out);
+        return LURK_OK;
+    });
+}
+
+int scale_affine(int curve_id, const uint8_t *xy, const uint8_t *r, int fmt, uint8_t out[64]) {
+    return dispatch_curve(curve_id, [&](auto c) {
+        uint8_t p96[96], q96[96];
+        affine_to_96<typename decltype(c)::Base>(xy, fmt, p96);
+        const uint8_t *pts[1] = {p96};
+        LURK_TRY(point_combination(curve_id, pts, r, 1, fmt, q96));
+        memcpy(out, q96, 64);                   // the identity is (0, 0) in both forms
+        return LURK_OK;
+    });
+}
+
 }  // namespace lurk
 
 using namespace lurk;
@@ -413,10 +485,9 @@ int lurk_ipa_prove_dev(int curve_id, lurk_msm_ctx *ck, const uint8_t ck_c[64], v
         set_error("commitment key: curve %d with %zu bases, need curve %d with >= 2^%d", ck_curve, ck_n, curve_id, log_n);
         return LURK_ERR_ARG;
     }
-    return dispatch_curve(curve_id, [&](auto c) {
-        return ipa_prove<decltype(c)>(ck, ck_c, d_a, d_b, log_n, challenge, user, L_out, R_out, a_final, b_final, fmt,
-                                      static_cast<cudaStream_t>(stream));
-    });
+    PcsArena arena;           // per call: allocated and freed as the prover goes, as always
+    return ipa_prove_arena(curve_id, ck, arena, ck_c, d_a, d_b, log_n, challenge, user, L_out, R_out, a_final, b_final, fmt,
+                           static_cast<cudaStream_t>(stream));
 }
 
 int lurk_ipa_verify_dev(int curve_id, lurk_msm_ctx *ck, const uint8_t ck_c[64], const uint8_t comm[96], const uint8_t c[32], const void *d_b,

@@ -9,6 +9,7 @@
 // go through the library's own Pippenger (lurk_msm_ctx_*) on device pointers.
 #include "common.cuh"
 #include "kzg.cuh"
+#include "pcs.cuh"
 #include "reduce.cuh"
 #include "sc_scratch.cuh"
 
@@ -215,7 +216,7 @@ static int kzg_witness_polys(const F *d_B, size_t n, const F u[3], F *d_h, DevBu
     size_t total = 0;
     std::vector<size_t> off(K + 1, 0);
     for (int k = 1; k <= K; k++) { off[k] = total; total += 3 * lens[k]; }
-    LURK_TRY(scratch.alloc(std::max<size_t>(total, 1) * sizeof(F)));
+    LURK_TRY(PcsArena::grow(scratch, std::max<size_t>(total, 1) * sizeof(F)));
     F *Y = scratch.as<F>();
     std::vector<Tri<F>> mult(K + 1);
     for (int y = 0; y < 3; y++) mult[0].v[y] = u[y];
@@ -239,8 +240,9 @@ static int kzg_witness_polys(const F *d_B, size_t n, const F u[3], F *d_h, DevBu
     return LURK_OK;
 }
 
+// Every buffer, clone, stream and event comes from the arena A, grown where the one-shot entry point allocated it.
 template <class C>
-static int hyperkzg_prove(lurk_msm_ctx *ck, const void *d_poly, const uint8_t *point, int l, lurk_challenge_fn challenge, void *user,
+static int hyperkzg_prove(lurk_msm_ctx *ck, PcsArena &A, const void *d_poly, const uint8_t *point, int l, lurk_challenge_fn challenge, void *user,
                           uint8_t *com_out, uint8_t *w_out, uint8_t *v_out, int fmt, cudaStream_t s) {
     using F = typename C::Scalar;
     const size_t n = (size_t)1 << l;
@@ -248,10 +250,9 @@ static int hyperkzg_prove(lurk_msm_ctx *ck, const void *d_poly, const uint8_t *p
     for (int i = 0; i < l; i++)
         if (!fe_in(point + 32 * i, fmt, x[i])) { set_error("point[%d] is not reduced", i); return LURK_ERR_RANGE; }
     // Phase 1: P_0 = the polynomial, P_{i+1}[j] = P_i[2j] + x[l-1-i] (P_i[2j+1] - P_i[2j]); commitments of P_1 .. P_{l-1}
-    DevBuf polys_buf;
-    LURK_TRY(polys_buf.alloc(2 * n * sizeof(F)));
-    F *polys = polys_buf.as<F>();
-    LURK_CUDA_TRY(cudaMemcpyAsync(polys, d_poly, n * sizeof(F), cudaMemcpyDeviceToDevice, s));
+    LURK_TRY(PcsArena::grow(A.polys, 2 * n * sizeof(F)));
+    F *polys = A.polys.as<F>();
+    if (d_poly != polys) LURK_CUDA_TRY(cudaMemcpyAsync(polys, d_poly, n * sizeof(F), cudaMemcpyDeviceToDevice, s));
     for (int i = 0; i + 1 < l; i++) {
         const size_t half = n >> (i + 1);
         kzg_fold_kernel<F><<<kzg_grid(half, 256), 256, 0, s>>>(polys + kzg_poly_offset(n, i), polys + kzg_poly_offset(n, i + 1), half, x[l - 1 - i]);
@@ -259,13 +260,11 @@ static int hyperkzg_prove(lurk_msm_ctx *ck, const void *d_poly, const uint8_t *p
     LURK_CUDA_TRY(cudaGetLastError());
     // the l - 1 commitments are independent and mostly short (latency-bound Pippenger chains): three of them in flight, on the context and
     // two clones of it (same resident key, own scratch), each on its own stream
-    MsmCloneGuard clone[2];
-    StreamGuard side[2];
-    EventGuard ready;
-    LURK_TRY(ready.create());
-    for (int k = 0; k < 2; k++) { LURK_TRY(lurk_msm_ctx_clone(ck, &clone[k].c)); LURK_TRY(side[k].create()); }
-    lurk_msm_ctx *ctxs[3] = {ck, clone[0].c, clone[1].c};
-    cudaStream_t streams[3] = {s, side[0].s, side[1].s};
+    LURK_TRY(A.event());
+    LURK_TRY(A.clones(ck, 2));
+    EventGuard &ready = A.ready;
+    lurk_msm_ctx *ctxs[3] = {ck, A.clone[0].c, A.clone[1].c};
+    cudaStream_t streams[3] = {s, A.side[0].s, A.side[1].s};
     LURK_CUDA_TRY(cudaEventRecord(ready.e, s));
     for (int k = 1; k < 3; k++) LURK_CUDA_TRY(cudaStreamWaitEvent(streams[k], ready.e, 0));
     std::vector<uint8_t> com((size_t)std::max(l - 1, 1) * 96);
@@ -300,11 +299,11 @@ static int hyperkzg_prove(lurk_msm_ctx *ck, const void *d_poly, const uint8_t *p
     }
     first[l] = (uint32_t)chunks.size();
     const size_t nchunks = chunks.size();
-    DevBuf d_chunks, d_first, d_partial, d_v;
-    LURK_TRY(d_chunks.alloc(nchunks * sizeof(EvalChunk)));
-    LURK_TRY(d_first.alloc((l + 1) * sizeof(uint32_t)));
-    LURK_TRY(d_partial.alloc(3 * nchunks * sizeof(F)));
-    LURK_TRY(d_v.alloc((size_t)3 * l * sizeof(F)));
+    DevBuf &d_chunks = A.chunks, &d_first = A.first, &d_partial = A.partial, &d_v = A.v;
+    LURK_TRY(PcsArena::grow(d_chunks, nchunks * sizeof(EvalChunk)));
+    LURK_TRY(PcsArena::grow(d_first, (l + 1) * sizeof(uint32_t)));
+    LURK_TRY(PcsArena::grow(d_partial, 3 * nchunks * sizeof(F)));
+    LURK_TRY(PcsArena::grow(d_v, (size_t)3 * l * sizeof(F)));
     LURK_CUDA_TRY(cudaMemcpyAsync(d_chunks.p, chunks.data(), nchunks * sizeof(EvalChunk), cudaMemcpyHostToDevice, s));
     LURK_CUDA_TRY(cudaMemcpyAsync(d_first.p, first.data(), (l + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     EvalArgs<F> ea;
@@ -329,9 +328,9 @@ static int hyperkzg_prove(lurk_msm_ctx *ck, const void *d_poly, const uint8_t *p
     ba.l = l;
     ba.qpow[0] = F::one();
     for (int j = 1; j < l; j++) ba.qpow[j] = ba.qpow[j - 1] * q;
-    DevBuf d_B, d_h, scan_scratch;
-    LURK_TRY(d_B.alloc(n * sizeof(F)));
-    LURK_TRY(d_h.alloc(3 * n * sizeof(F)));
+    DevBuf &d_B = A.B, &d_h = A.h, &scan_scratch = A.scan;
+    LURK_TRY(PcsArena::grow(d_B, n * sizeof(F)));
+    LURK_TRY(PcsArena::grow(d_h, 3 * n * sizeof(F)));
     kzg_batch_kernel<F><<<kzg_grid(n, 256), 256, 0, s>>>(polys, n, ba, d_B.as<F>());
     LURK_CUDA_TRY(cudaGetLastError());
     LURK_TRY(kzg_witness_polys<F>(d_B.as<F>(), n, u, d_h.as<F>(), scan_scratch, s));
@@ -346,6 +345,13 @@ static int hyperkzg_prove(lurk_msm_ctx *ck, const void *d_poly, const uint8_t *p
     rc = challenge(user, 2, w, sizeof w, ignored);       // keeps the caller's transcript in the verifier's state
     if (rc != 0) { set_error("challenge callback failed (witness commitments, %d)", rc); return LURK_ERR_ARG; }
     return LURK_OK;
+}
+
+int hyperkzg_prove_arena(int curve_id, lurk_msm_ctx *ck, PcsArena &a, const void *d_poly, const uint8_t *point, int l, lurk_challenge_fn challenge,
+                         void *user, uint8_t *com_out, uint8_t *w_out, uint8_t *v_out, int fmt, cudaStream_t s) {
+    return dispatch_curve(curve_id, [&](auto c) {
+        return hyperkzg_prove<decltype(c)>(ck, a, d_poly, point, l, challenge, user, com_out, w_out, v_out, fmt, s);
+    });
 }
 
 }  // namespace lurk
@@ -374,9 +380,8 @@ int lurk_hyperkzg_prove_dev(int curve_id, lurk_msm_ctx *ck, const void *d_poly, 
         set_error("commitment key: curve %d with %zu bases, need curve %d with >= 2^%d", ck_curve, ck_n, curve_id, num_vars);
         return LURK_ERR_ARG;
     }
-    return dispatch_curve(curve_id, [&](auto c) {
-        return hyperkzg_prove<decltype(c)>(ck, d_poly, point, num_vars, challenge, user, com_out, w_out, v_out, fmt, static_cast<cudaStream_t>(stream));
-    });
+    PcsArena arena;           // per call: allocated and freed as the prover goes, as always
+    return hyperkzg_prove_arena(curve_id, ck, arena, d_poly, point, num_vars, challenge, user, com_out, w_out, v_out, fmt, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -1,0 +1,51 @@
+// The opening provers' scratch (HyperKZG: kzg.cu, the inner-product argument: ipa.cu) as an object the caller can keep, and the host
+// point arithmetic the compress context (compress.cu) needs around them.  lurk_hyperkzg_prove_dev / lurk_ipa_prove_dev build a fresh
+// arena per call, so they allocate what they always did, where they always did; lurk_compress_ctx keeps one per circuit, grown by its
+// first proof and reused by every later one (no cudaMalloc / cudaFree, no stream or clone creation on the proving path).
+#pragma once
+#include "common.cuh"
+#include "sc_scratch.cuh"
+
+namespace lurk {
+
+struct PcsArena {
+    // declared in the order the one-shot HyperKZG prover created them, so that they are released in the order it released them
+    DevBuf polys;                 // HyperKZG: the fold chain P_0 | P_1 | .. (2n);  compress's IPA: a (n) | b (n)
+    MsmCloneGuard clone[2];       // clones of the key context (own scratch, same resident key): HyperKZG 2, IPA 1
+    StreamGuard side[2];
+    EventGuard ready;
+    DevBuf chunks, first, partial, v;     // HyperKZG: the evaluation chunks and their partial sums
+    DevBuf B, h, scan;            // HyperKZG: the batched polynomial (n), the witness polynomials (3n), the up-sweep levels
+    DevBuf weights;               // IPA: the key weights W | sl | sr (3n)
+    // the buffer holds at least `bytes`; a fresh DevBuf gets exactly `bytes` (what the one-shot entry points allocated)
+    static int grow(DevBuf &b, size_t bytes) { return b.bytes >= bytes ? LURK_OK : b.alloc(bytes); }
+    int clones(lurk_msm_ctx *ck, int k) {
+        for (int i = 0; i < k; i++) {
+            if (!clone[i].c) LURK_TRY(lurk_msm_ctx_clone(ck, &clone[i].c));
+            if (!side[i].s) LURK_TRY(side[i].create());
+        }
+        return LURK_OK;
+    }
+    int event() { return ready.e ? LURK_OK : ready.create(); }
+    size_t device_bytes() const {
+        return polys.bytes + B.bytes + h.bytes + scan.bytes + chunks.bytes + first.bytes + partial.bytes + v.bytes + weights.bytes;
+    }
+};
+
+// provider::hyperkzg::EvaluationEngine::prove on the arena; d_poly may be the arena's P_0 (the joint polynomial written in place), then
+// the copy into P_0 is skipped.  `ck` has been checked by the caller (curve, >= 2^l bases).
+int hyperkzg_prove_arena(int curve_id, lurk_msm_ctx *ck, PcsArena &a, const void *d_poly, const uint8_t *point, int l, lurk_challenge_fn challenge,
+                         void *user, uint8_t *com_out, uint8_t *w_out, uint8_t *v_out, int fmt, cudaStream_t s);
+// InnerProductArgument::prove's rounds on the arena; d_a / d_b consumed as by lurk_ipa_prove_dev
+int ipa_prove_arena(int curve_id, lurk_msm_ctx *ck, PcsArena &a, const uint8_t *gc_bytes, void *d_a, void *d_b, int log_n, lurk_challenge_fn challenge,
+                    void *user, uint8_t *L_out, uint8_t *R_out, uint8_t *a_final, uint8_t *b_final, int fmt, cudaStream_t s);
+// every 96-byte point x | y | z of the header's form (z = 1 on the curve, or the identity 0 | 0 | 0), in `fmt`; host only
+bool points_valid(int curve_id, const uint8_t *const *points, int count, int fmt);
+// an affine point x | y (identity = (0, 0)) of the curve, in `fmt`; host only
+bool affine_valid(int curve_id, const uint8_t *xy, int fmt);
+// out = sum_k scalars[k] points[k] (points as points_valid takes them, scalars 32 bytes each), a 96-byte point in `fmt`; host only
+int point_combination(int curve_id, const uint8_t *const *points, const uint8_t *scalars, int count, int fmt, uint8_t out[96]);
+// r ck_c for the affine ck_c (x | y, `fmt`) and the scalar r (`fmt`) as an affine x | y in `fmt`; host only
+int scale_affine(int curve_id, const uint8_t *xy, const uint8_t *r, int fmt, uint8_t out[64]);
+
+}  // namespace lurk

@@ -564,6 +564,12 @@ static int spartan_prove(int n, lurk_spartan_ctx *const *ctxs, const void *const
     return LURK_OK;
 }
 
+// the prover behind lurk_spartan_prove_dev / _batch_dev for compress.cu, whose arguments its own checks have covered
+int spartan_prove_checked(int n, lurk_spartan_ctx *const *ctxs, const void *const *d_z, const void *const *d_E, lurk_spartan_challenge_fn fn, void *user,
+                          lurk_spartan_proof *out, void *d_joint, int fmt, cudaStream_t s, bool batched) {
+    return dispatch_field(ctxs[0]->field_id, [&](auto f) { return spartan_prove<decltype(f)>(n, ctxs, d_z, d_E, fn, user, out, d_joint, fmt, s, batched); });
+}
+
 // ------------------------------------------------------------------------------------------------ the verifier
 template <class F>
 static F pow2(int k) { F r = F::one(); const F two = F::from_u64(2); for (int j = 0; j < k; j++) r = r * two; return r; }

@@ -473,23 +473,28 @@ class BatchedRelaxedR1CSProver:
 
 
 # ------------------------------------------------------------------------------------------------ the Spartan prover context
+_SPARTAN_LABELS = {_capi.SPARTAN_OUTER: "outer", _capi.SPARTAN_INNER: "inner", _capi.SPARTAN_BATCH_EVAL: "batch_eval"}
+
+
+def _spartan_label(phase, rnd, msg, n, batched):
+    """(label, data) of one call of the phase-tagged transcript for challenge(label, data); msg: the message bytes"""
+    vals = _ints(np.frombuffer(msg, dtype=np.uint8)) if msg else []
+    if phase == _capi.SPARTAN_TAU:
+        return "tau", n if batched else rnd
+    if phase == _capi.SPARTAN_OUTER_R:
+        return "outer_r", n
+    if phase == _capi.SPARTAN_CLAIMS:
+        claims = tuple(tuple(vals[4 * i:4 * i + 4]) for i in range(n))
+        return "inner_r", claims if batched else claims[0]
+    return _SPARTAN_LABELS[phase], (rnd, vals)
+
+
 def _spartan_callback(challenge, p, n, batched, errors):
     """the phase-tagged transcript of lurk_spartan_prove_*_dev mapped onto the labels and data RelaxedR1CSProver, BatchedRelaxedR1CSProver and
     tests/batched_oracle.py use, so that one challenge(label, data) function drives every path"""
-    labels = {_capi.SPARTAN_OUTER: "outer", _capi.SPARTAN_INNER: "inner", _capi.SPARTAN_BATCH_EVAL: "batch_eval"}
-
     def cb(user, phase, rnd, msg, msg_len, out):
         try:
-            vals = _ints(np.frombuffer(C.string_at(msg, msg_len), dtype=np.uint8)) if msg_len else []
-            if phase == _capi.SPARTAN_TAU:
-                x = challenge("tau", n if batched else rnd)
-            elif phase == _capi.SPARTAN_OUTER_R:
-                x = challenge("outer_r", n)
-            elif phase == _capi.SPARTAN_CLAIMS:
-                claims = tuple(tuple(vals[4 * i:4 * i + 4]) for i in range(n))
-                x = challenge("inner_r", claims if batched else claims[0])
-            else:
-                x = challenge(labels[phase], (rnd, vals))
+            x = challenge(*_spartan_label(phase, rnd, C.string_at(msg, msg_len) if msg_len else b"", n, batched))
             for i, byte in enumerate((int(x) % p).to_bytes(32, "little")):
                 out[i] = byte
             return 0
