@@ -308,6 +308,12 @@ int lurk_batch_eval_reduce_dev(int field_id, int n_claims, const void *const *d_
 typedef struct lurk_spartan_ctx lurk_spartan_ctx;
 int lurk_spartan_ctx_create(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n_rows, const uint64_t *const row_ptr[3],
                             const uint32_t *const col[3], const uint8_t *const val[3], int fmt, lurk_spartan_ctx **out);
+/* A verifier-only context: the same arguments and checks, the three CSRs uploaded and range-checked, but no merged transpose,
+ * eval-table slots or tickets (the prover's).  lurk_spartan_matrix_evals_dev, lurk_spartan_verify, lurk_spartan_verify_batch and
+ * lurk_recursive_verify(_dev) take it and give exactly what a full context gives; lurk_spartan_prove_dev, _prove_batch_dev,
+ * _eval_table_dev and lurk_compress_ctx_create refuse it with LURK_ERR_ARG.  Destroyed by lurk_spartan_ctx_destroy. */
+int lurk_spartan_ctx_create_verifier(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n_rows, const uint64_t *const row_ptr[3],
+                                     const uint32_t *const col[3], const uint8_t *const val[3], int fmt, lurk_spartan_ctx **out);
 void lurk_spartan_ctx_destroy(lurk_spartan_ctx *ctx);
 /* any output may be NULL */
 int lurk_spartan_ctx_info(lurk_spartan_ctx *ctx, int *field_id, int *log_rows, int *log_vars, size_t *joint_len);
@@ -384,6 +390,42 @@ int lurk_spartan_verify(lurk_spartan_ctx *ctx, const uint8_t u[32], const uint8_
  * instance i's n_x_i x 32 bytes.  One matrix-evaluation launch per instance and one synchronisation. */
 int lurk_spartan_verify_batch(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u, const uint8_t *const *X, lurk_spartan_proof *proof,
                               int rounds_fmt, lurk_spartan_challenge_fn challenge, void *user, int *accepted, int fmt, void *stream);
+
+/* The satisfiability checks of RecursiveSNARK::verify (Proof::verify on a Recursive proof, src/proof/nova.rs:358-373,
+ * supernova.rs:304-317) in one call: R1CSShape::is_sat_relaxed on every running instance and is_sat on the secondary's last fresh
+ * instance.  Per instance, one pass over the shape's rows forms A z, B z, C z in registers and counts the rows where
+ * (A z)∘(B z) != u (C z) + E (no O(rows) scratch), then commit(W) and commit(E) are recomputed on the key and compared with comm_W and
+ * comm_E.  One call covers one proof: Nova [r_U_primary, r_U_secondary, l_u_secondary]; SuperNova every Some running primary, then the
+ * secondary's two instances.  n = 1..32.  Shapes and keys may repeat.
+ *
+ * The RO hashes (num_steps, z0, the two hashes compared with l_u_secondary.X) stay with the caller. */
+typedef struct lurk_recursive_instance {
+    lurk_spartan_ctx *shape;  /* full or verifier-only; borrowed                                                              */
+    lurk_msm_ctx *ck;         /* key on the curve whose scalar field is the shape's field, >= max(n_w, n_rows) bases; not consumed */
+    const void *z;            /* (W, u, X): n_w + 1 + n_x elements, laid out as LURK_FOLD_BUF_Z1 / LURK_FOLD_BUF_W2 hold it     */
+    const void *E;            /* n_rows elements; NULL = strict instance (R1CSShape::is_sat: the u slot must hold 1)          */
+    const uint8_t *comm_W;    /* 96 bytes, `fmt`, x | y | 1 or 0 | 0 | 0 for the identity                                     */
+    const uint8_t *comm_E;    /* 96 bytes as comm_W; NULL exactly when E is NULL                                              */
+} lurk_recursive_instance;
+typedef struct lurk_recursive_verdict {
+    uint64_t bad_rows;        /* rows where the R1CS equation fails                                                           */
+    uint64_t first_bad_row;   /* the first of them; UINT64_MAX when every row holds                                           */
+    int u_ok;                 /* strict: u == 1; relaxed: 1                                                                   */
+    int comm_W_ok, comm_E_ok; /* the recomputed commitments equal the given ones; comm_E_ok = 1 for a strict instance          */
+} lurk_recursive_verdict;
+/* _dev: z and E are Montgomery elements on the device, as the fold contexts hold them (LURK_FOLD_BUF_Z1 / _E1 for a running instance,
+ * LURK_FOLD_BUF_W2 for a staged fresh one); `fmt` applies to the commitments only.  The host form: z and E are host memory in `fmt`,
+ * uploaded into stream-ordered scratch and converted there.  Neither form writes the caller's vectors.
+ * *accepted = 1 when every verdict holds (bad_rows == 0, u_ok, comm_W_ok, comm_E_ok); a rejected proof is LURK_OK with *accepted = 0 and
+ * every verdict filled in.  An element of z or E >= p, or a commitment off the curve, is LURK_ERR_RANGE; null pointers, n out of range,
+ * E without comm_E or the reverse, a key that is too short, on another device or on the curve of another field are LURK_ERR_ARG.  Every
+ * argument check runs before any device work.
+ * Each distinct key context gets a stream forked from `stream` and joined before the call returns, so the primary's and the secondary's
+ * instances run at once; on its stream each instance runs the R1CS pass, commit(W), then commit(E), through lurk_msm_ctx_launch_dev /
+ * _finish on the borrowed key.  Synchronous.  The key contexts must have no launch pending and must not be used concurrently by the
+ * caller during the call. */
+int lurk_recursive_verify_dev(int n, const lurk_recursive_instance *inst, lurk_recursive_verdict *out, int *accepted, int fmt, void *stream);
+int lurk_recursive_verify(int n, const lurk_recursive_instance *inst, lurk_recursive_verdict *out, int *accepted, int fmt, void *stream);
 
 /* Compress context: CompressedSNARK::prove (Nova's `compress`, src/proof/nova.rs:341-356; SuperNova's, supernova.rs:293-317) in one call
  * -- for the primary and the secondary circuit, RelaxedR1CSSNARK::prove (or BatchedRelaxedR1CSSNARK::prove for SuperNova's primary),

@@ -60,6 +60,17 @@ pub struct lurk_compress_proof { pub primary: lurk_compress_circuit_proof, pub s
 /// primary, 1 = secondary; the two circuits' calls may come from two threads at once (one transcript per circuit).
 pub type lurk_compress_challenge_fn = unsafe extern "C" fn(user: *mut c_void, circuit: c_int, phase: c_int, round: c_int, message: *const u8,
                                                            message_len: usize, challenge_out: *mut u8) -> c_int;
+/// one instance of RecursiveSNARK::verify's is_sat checks (include/lurk_b200.h: lurk_recursive_instance); e / comm_e null for a strict
+/// instance (l_u_secondary)
+#[repr(C)]
+pub struct lurk_recursive_instance {
+    pub shape: *mut lurk_spartan_ctx, pub ck: *mut lurk_msm_ctx, pub z: *const c_void, pub e: *const c_void, pub comm_w: *const u8,
+    pub comm_e: *const u8,
+}
+/// what one instance's checks found: first_bad_row = u64::MAX when every row holds
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct lurk_recursive_verdict { pub bad_rows: u64, pub first_bad_row: u64, pub u_ok: c_int, pub comm_w_ok: c_int, pub comm_e_ok: c_int }
 #[repr(C)]
 #[derive(Clone, Copy)]
 pub struct lurk_dag_node { pub kind: u8, pub reserved: u8, pub tag: [u16; 4], pub child: [u32; 4] }
@@ -136,6 +147,8 @@ extern "C" {
     // N4 -- RelaxedR1CSSNARK::prove / BatchedRelaxedR1CSSNARK::prove in one call (src/proof/nova.rs:341-356, supernova.rs:293-317)
     pub fn lurk_spartan_ctx_create(field_id: c_int, n_w: u64, n_x: u64, n_rows: u64, row_ptr: *const *const u64, col: *const *const u32,
                                    val: *const *const u8, fmt: c_int, out: *mut *mut lurk_spartan_ctx) -> c_int;
+    pub fn lurk_spartan_ctx_create_verifier(field_id: c_int, n_w: u64, n_x: u64, n_rows: u64, row_ptr: *const *const u64, col: *const *const u32,
+                                            val: *const *const u8, fmt: c_int, out: *mut *mut lurk_spartan_ctx) -> c_int;
     pub fn lurk_spartan_ctx_destroy(ctx: *mut lurk_spartan_ctx);
     pub fn lurk_spartan_ctx_info(ctx: *mut lurk_spartan_ctx, field_id: *mut c_int, log_rows: *mut c_int, log_vars: *mut c_int, joint_len: *mut usize) -> c_int;
     pub fn lurk_spartan_prove_dev(ctx: *mut lurk_spartan_ctx, d_z: *const c_void, d_e: *const c_void, challenge: lurk_spartan_challenge_fn, user: *mut c_void,
@@ -155,6 +168,13 @@ extern "C" {
     pub fn lurk_ipa_verify_dev(curve_id: c_int, ck: *mut lurk_msm_ctx, ck_c: *const u8, comm: *const u8, c: *const u8, d_b: *const c_void, log_n: c_int,
                                l: *const u8, r: *const u8, a_final: *const u8, challenge: lurk_challenge_fn, user: *mut c_void, accepted: *mut c_int,
                                ck_hat_out: *mut u8, b_hat_out: *mut u8, fmt: c_int, stream: *mut c_void) -> c_int;
+    // S6 -- RecursiveSNARK::verify's three is_sat* calls (Proof::verify on a Recursive proof, src/proof/nova.rs:358-373): Nova
+    // [r_U_primary, r_U_secondary, l_u_secondary], SuperNova every Some running primary then the secondary's two.  The num_steps, z0 and
+    // X.len() checks and the two RO hashes stay in Rust.  Host form: z = (W, u, X) and E as Arecibo's structs hold them, in `fmt`.
+    pub fn lurk_recursive_verify(n: c_int, inst: *const lurk_recursive_instance, out: *mut lurk_recursive_verdict, accepted: *mut c_int, fmt: c_int,
+                                 stream: *mut c_void) -> c_int;
+    pub fn lurk_recursive_verify_dev(n: c_int, inst: *const lurk_recursive_instance, out: *mut lurk_recursive_verdict, accepted: *mut c_int,
+                                     fmt: c_int, stream: *mut c_void) -> c_int;
     // CompressedSNARK::prove in one call.  Before it, fold l_u_secondary into r_U_secondary (Arecibo's NIFS::prove) with one more
     // lurk_fold_ctx_stage_a + lurk_fold_ctx_stage_b_launch + lurk_fold_ctx_collect on the secondary fold context; then pass both fold
     // contexts' LURK_FOLD_BUF_Z1 / _E1 pointers and the records' running commitments.

@@ -81,6 +81,15 @@ class CompressProof(C.Structure):
     _fields_ = [("primary", CompressCircuitProof), ("secondary", CompressCircuitProof)]
 
 
+# the recursive verifier (lurk_recursive_verify, _dev)
+class RecursiveInstance(C.Structure):
+    _fields_ = [(name, C.c_void_p) for name in ("shape", "ck", "z", "E", "comm_W", "comm_E")]
+
+
+class RecursiveVerdict(C.Structure):
+    _fields_ = [("bad_rows", C.c_uint64), ("first_bad_row", C.c_uint64), ("u_ok", C.c_int), ("comm_W_ok", C.c_int), ("comm_E_ok", C.c_int)]
+
+
 # every symbol declared in include/lurk_b200.h: name -> (restype, argtypes)
 PROTOTYPES = {
     "lurk_last_error": (C.c_char_p, []),
@@ -134,6 +143,7 @@ PROTOTYPES = {
     "lurk_hyperkzg_prove_dev": (_i, [_i, _vp, _vp, _vp, _i, CHALLENGE_FN, _vp, _vp, _vp, _vp, _i, _vp]),
     "lurk_batch_eval_reduce_dev": (_i, [_i, _i, C.POINTER(_vp), C.POINTER(_i), _vp, _vp, CHALLENGE_FN, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     "lurk_spartan_ctx_create": (_i, [_i, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _i, C.POINTER(_vp)]),
+    "lurk_spartan_ctx_create_verifier": (_i, [_i, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _i, C.POINTER(_vp)]),
     "lurk_spartan_ctx_destroy": (None, [_vp]),
     "lurk_spartan_ctx_info": (_i, [_vp, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), C.POINTER(_sz)]),
     "lurk_spartan_prove_dev": (_i, [_vp, _vp, _vp, SPARTAN_CHALLENGE_FN, _vp, C.POINTER(SpartanProof), _vp, _i, _vp]),
@@ -149,6 +159,8 @@ PROTOTYPES = {
     "lurk_compress_ctx_info": (_i, [_vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "lurk_compress_prove_dev": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _vp, _vp, _vp, _vp, COMPRESS_CHALLENGE_FN, _vp, _i,
                                      C.POINTER(CompressProof), _i, _vp]),
+    "lurk_recursive_verify_dev": (_i, [_i, C.POINTER(RecursiveInstance), C.POINTER(RecursiveVerdict), C.POINTER(_i), _i, _vp]),
+    "lurk_recursive_verify": (_i, [_i, C.POINTER(RecursiveInstance), C.POINTER(RecursiveVerdict), C.POINTER(_i), _i, _vp]),
     "lurk_ipa_verify_dev": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, CHALLENGE_FN, _vp, C.POINTER(_i), _vp, _vp, _i, _vp]),
     "lurk_axpy_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp]),
     "lurk_spmv_csr_dev": (_i, [_i, _vp, _vp, _vp, _sz, _vp, _vp, _vp]),

@@ -21,6 +21,7 @@ namespace lurk {
 
 int spartan_prove_checked(int n, lurk_spartan_ctx *const *ctxs, const void *const *d_z, const void *const *d_E, lurk_spartan_challenge_fn fn, void *user,
                           lurk_spartan_proof *out, void *d_joint, int fmt, cudaStream_t s, bool batched);     // spartan.cu
+int refuse_verifier_only(const lurk_spartan_ctx *ctx, const char *who);                                       // spartan.cu
 
 constexpr int CP_MAX_PRIMARY = 30;
 
@@ -216,6 +217,8 @@ int lurk_compress_ctx_create(int n_primary, lurk_spartan_ctx *const *primary, lu
             if (primary[k] == primary[i]) { set_error("primary contexts %d and %d are the same context", k, i); return LURK_ERR_ARG; }
     }
     if (pcs_primary->ck == pcs_secondary->ck) { set_error("the primary and the secondary key are the same context"); return LURK_ERR_ARG; }
+    for (int i = 0; i < n_primary; i++) LURK_TRY(refuse_verifier_only(primary[i], "lurk_compress_ctx_create (primary)"));
+    LURK_TRY(refuse_verifier_only(secondary, "lurk_compress_ctx_create (secondary)"));
     LURK_TRY(require_gpu());
     lurk_compress_ctx *ctx = new lurk_compress_ctx();
     int rc = check_circuit("primary", n_primary, primary, pcs_primary, fmt, ctx->c[0]);

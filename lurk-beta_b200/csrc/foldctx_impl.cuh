@@ -75,27 +75,6 @@ __global__ void __launch_bounds__(256) fold_axpy_kernel(FoldAxpyArgs<F> a, const
     }
 }
 
-// relaxed R1CS residual: counts rows with az*bz != u*cz + e; with `kept` vectors (the incrementally folded A z, B z, C z) also
-// rows where those differ from the freshly computed products
-template <class F>
-__global__ void __launch_bounds__(256) relaxed_residual_kernel(const F *__restrict__ az, const F *__restrict__ bz, const F *__restrict__ cz,
-                                                               const F *__restrict__ e, const F *__restrict__ up, const F *__restrict__ kept_a,
-                                                               const F *__restrict__ kept_b, const F *__restrict__ kept_c, size_t n,
-                                                               unsigned long long *bad) {
-    const F u = load_fe<F>(up);
-    unsigned local = 0;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const F a = load_fe<F>(az + i), b = load_fe<F>(bz + i), c = load_fe<F>(cz + i);
-        const F lhs = a * b;
-        const F rhs = u * c + load_fe<F>(e + i);
-        bool ok = lhs == rhs;
-        if (kept_a) ok = ok && a == load_fe<F>(kept_a + i) && b == load_fe<F>(kept_b + i) && c == load_fe<F>(kept_c + i);
-        local += ok ? 0u : 1u;
-    }
-    local = __reduce_add_sync(0xffffffffu, local);
-    if ((threadIdx.x & 31) == 0 && local) atomicAdd(bad, (unsigned long long)local);
-}
-
 // strided element-wise conversion (canonical -> Montgomery) of the spans of W2 the host fills
 template <class F>
 __global__ void __launch_bounds__(256) span_to_mont_kernel(F *base, uint64_t first, uint64_t row_elems, uint64_t stride, uint64_t rows) {

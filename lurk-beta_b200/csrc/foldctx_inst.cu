@@ -291,7 +291,7 @@ struct FoldCtx final : FoldCtxBase {
         LURK_CUDA_TRY(cudaMemset(seq_dev.p, 0, sizeof(unsigned long long)));
         LURK_TRY(run_pts.alloc(2 * sizeof(Pt)));
         LURK_CUDA_TRY(cudaMemset(run_pts.p, 0, 2 * sizeof(Pt)));
-        LURK_TRY(bad_dev.alloc(sizeof(unsigned long long)));
+        LURK_TRY(bad_dev.alloc(sizeof(SatCount)));
         LURK_TRY(xchg.alloc(sizeof(XchgBuf<Fb>)));
         LURK_CUDA_TRY(cudaMemset(xchg.p, 0, sizeof(XchgBuf<Fb>)));
         peers[c.rank] = xchg.as<XchgBuf<Fb>>();
@@ -788,21 +788,11 @@ struct FoldCtx final : FoldCtxBase {
         LURK_TRY(need_peers());
         LURK_TRY(sync());
         const size_t rows = cfg.n_rows;
-        unsigned long long bad = 0;
-        if (rows) {
-            // fresh A z, B z, C z into scratch; the vectors kept current by the folds (mv1) must equal them
-            Fs *fresh = nullptr;
-            LURK_CUDA_TRY(cudaMallocAsync((void **)&fresh, 3 * rows * sizeof(Fs), sB));
-            LURK_CUDA_TRY(cudaMemsetAsync(bad_dev.p, 0, sizeof(unsigned long long), sB));
-            spmv3_kernel<Fs><<<dim3(fold_grid(rows, 256, 8), 3), 256, 0, sB>>>(csr[0], csr[1], csr[2], rows, z1.as<Fs>(), fresh, fresh + rows, fresh + 2 * rows);
-            relaxed_residual_kernel<Fs><<<fold_grid(rows, 256, 8), 256, 0, sB>>>(fresh, fresh + rows, fresh + 2 * rows, e1.as<Fs>(), z1.as<Fs>() + cfg.n_w,
-                                                                                mv1_valid ? mv1[0].as<Fs>() : nullptr, mv1[1].as<Fs>(), mv1[2].as<Fs>(), rows,
-                                                                                bad_dev.as<unsigned long long>());
-            cudaError_t e = cudaGetLastError();
-            cudaFreeAsync(fresh, sB);
-            LURK_CUDA_TRY(e);
-            LURK_CUDA_TRY(cudaMemcpyAsync(&bad, bad_dev.p, sizeof bad, cudaMemcpyDeviceToHost, sB));
-        }
+        // one pass with the products in registers; the vectors kept current by the folds (mv1) must equal the fresh products
+        const Fs *kept[3] = {mv1[0].as<Fs>(), mv1[1].as<Fs>(), mv1[2].as<Fs>()};
+        SatCount cnt{0, 0};
+        LURK_TRY(r1cs_sat_launch<Fs>(csr, rows, z1.as<Fs>(), cfg.n_w, e1.as<Fs>(), mv1_valid ? kept : nullptr, bad_dev.as<SatCount>(), sB));
+        LURK_CUDA_TRY(cudaMemcpyAsync(&cnt, bad_dev.p, sizeof cnt, cudaMemcpyDeviceToHost, sB));     // read after the synchronisation of sB below
         // commit(W1) with the W key, commit(E1) with the T key, exchanged and normalised like a step's commitments
         LURK_TRY(msm_launch<C>(ckChkW, z1.p, cfg.n_w, LURK_FMT_MONTGOMERY, sB, false));
         LURK_TRY(msm_launch<C>(ckChk, e1.p, rows, LURK_FMT_MONTGOMERY, sB, false));
@@ -827,7 +817,7 @@ struct FoldCtx final : FoldCtxBase {
         point_bytes(r.ct_x, r.ct_y, r.ct_inf, LURK_FMT_MONTGOMERY, have);
         point_to_bytes(pts[1], LURK_FMT_MONTGOMERY, want);
         if (comm_e_ok) *comm_e_ok = memcmp(have, want, 96) == 0;
-        if (bad_rows) *bad_rows = bad;
+        if (bad_rows) *bad_rows = cnt.bad;
         return LURK_OK;
     }
 

@@ -275,6 +275,7 @@ struct lurk_spartan_ctx {
     int field_id = 0;
     uint64_t n_w = 0, n_x = 0, rows = 0, num_vars = 0;
     int log_rows = 0, log_vars = 0;
+    bool verifier_only = false;  // the three CSRs only: no merged transpose, eval-table slots or tickets
     virtual ~lurk_spartan_ctx() {}
     size_t z_len() const { return n_w + 1 + n_x; }
 };
@@ -320,6 +321,10 @@ struct SpartanCtx : lurk_spartan_ctx {
             csr[m].val = val[m].p;
             this->nnz[m] = nnz;
             tnnz += nnz;
+        }
+        if (verifier_only) {
+            LURK_CUDA_TRY(cudaStreamSynchronize(s));     // the conversions above
+            return LURK_OK;
         }
         // merged transpose over the padded z's 2 num_vars columns
         const size_t trows = 2 * num_vars;
@@ -790,6 +795,30 @@ static int spartan_verify(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u
 
 static int ceil_log2(uint64_t x) { int l = 0; while (((uint64_t)1 << l) < x) l++; return l; }
 
+namespace lurk {
+
+// the prover's calls need the merged transpose a verifier-only context does not build
+int refuse_verifier_only(const lurk_spartan_ctx *ctx, const char *who) {
+    if (!ctx->verifier_only) return LURK_OK;
+    set_error("%s needs a full Spartan context; this one was made by lurk_spartan_ctx_create_verifier, which keeps no transpose", who);
+    return LURK_ERR_ARG;
+}
+
+// what the recursive verifier (recursive.cu) reads of a shape: sizes, field and the three device CSRs
+void spartan_ctx_shape(const lurk_spartan_ctx *ctx, int *field_id, uint64_t *n_w, uint64_t *n_x, uint64_t *rows, CsrDev csr[3]) {
+    *field_id = ctx->field_id;
+    *n_w = ctx->n_w;
+    *n_x = ctx->n_x;
+    *rows = ctx->rows;
+    dispatch_field(ctx->field_id, [&](auto f) {
+        const SpartanCtx<decltype(f)> *c = static_cast<const SpartanCtx<decltype(f)> *>(ctx);
+        for (int m = 0; m < 3; m++) csr[m] = c->csr[m];
+        return LURK_OK;
+    });
+}
+
+}  // namespace lurk
+
 static bool overlaps(const void *a, size_t a_bytes, const void *b, size_t b_bytes) {
     const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
     return a0 < b0 + b_bytes && b0 < a0 + a_bytes;
@@ -807,6 +836,7 @@ static int check_prove_args(int n, lurk_spartan_ctx *const *ctxs, const void *co
     int m = 0;
     for (int i = 0; i < n; i++) {
         if (!ctxs[i]) { set_error("null context %d", i); return LURK_ERR_ARG; }
+        LURK_TRY(refuse_verifier_only(ctxs[i], "the prover"));
         if (!d_z[i] || !d_E[i]) { set_error("null d_z / d_E of instance %d", i); return LURK_ERR_ARG; }
         if (ctxs[i]->field_id != ctxs[0]->field_id) {
             set_error("context %d is over field %d, context 0 over field %d", i, ctxs[i]->field_id, ctxs[0]->field_id);
@@ -852,10 +882,8 @@ static int check_verify_args(int n, lurk_spartan_ctx *const *ctxs, const uint8_t
     return LURK_OK;
 }
 
-extern "C" {
-
-int lurk_spartan_ctx_create(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n_rows, const uint64_t *const row_ptr[3], const uint32_t *const col[3],
-                            const uint8_t *const val[3], int fmt, lurk_spartan_ctx **out) {
+static int spartan_ctx_create(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n_rows, const uint64_t *const row_ptr[3], const uint32_t *const col[3],
+                              const uint8_t *const val[3], int fmt, bool verifier_only, lurk_spartan_ctx **out) {
     if (!out) { set_error("null out"); return LURK_ERR_ARG; }
     *out = nullptr;
     if (!row_ptr || !col || !val) { set_error("null matrix arrays"); return LURK_ERR_ARG; }
@@ -884,6 +912,7 @@ int lurk_spartan_ctx_create(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n
         c->log_rows = std::max(1, ceil_log2(n_rows));
         c->log_vars = std::max(1, ceil_log2(std::max(n_w, n_x + 1)));
         c->num_vars = (uint64_t)1 << c->log_vars;
+        c->verifier_only = verifier_only;
         const int r = c->init(row_ptr, col, val, fmt);
         if (r != LURK_OK) { delete c; return r; }
         ctx = c;
@@ -892,6 +921,18 @@ int lurk_spartan_ctx_create(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n
     if (rc != LURK_OK) return rc;
     *out = ctx;
     return LURK_OK;
+}
+
+extern "C" {
+
+int lurk_spartan_ctx_create(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n_rows, const uint64_t *const row_ptr[3], const uint32_t *const col[3],
+                            const uint8_t *const val[3], int fmt, lurk_spartan_ctx **out) {
+    return spartan_ctx_create(field_id, n_w, n_x, n_rows, row_ptr, col, val, fmt, false, out);
+}
+
+int lurk_spartan_ctx_create_verifier(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n_rows, const uint64_t *const row_ptr[3],
+                                     const uint32_t *const col[3], const uint8_t *const val[3], int fmt, lurk_spartan_ctx **out) {
+    return spartan_ctx_create(field_id, n_w, n_x, n_rows, row_ptr, col, val, fmt, true, out);
 }
 
 void lurk_spartan_ctx_destroy(lurk_spartan_ctx *ctx) { delete ctx; }
@@ -928,6 +969,7 @@ int lurk_spartan_prove_dev(lurk_spartan_ctx *ctx, const void *d_z, const void *d
 int lurk_spartan_eval_table_dev(lurk_spartan_ctx *ctx, const void *d_eq_rx, const uint8_t r[32], void *d_out, int fmt, void *stream) {
     if (!ctx || !d_eq_rx || !r || !d_out) { set_error("null argument"); return LURK_ERR_ARG; }
     if (fmt != LURK_FMT_CANONICAL && fmt != LURK_FMT_MONTGOMERY) { set_error("bad format %d", fmt); return LURK_ERR_ARG; }
+    LURK_TRY(refuse_verifier_only(ctx, "lurk_spartan_eval_table_dev"));
     LURK_TRY(require_gpu());
     return dispatch_field(ctx->field_id, [&](auto f) {
         using F = decltype(f);

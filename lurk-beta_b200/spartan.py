@@ -507,10 +507,12 @@ def _spartan_callback(challenge, p, n, batched, errors):
 class SpartanContext:
     """lurk_spartan_ctx: one circuit shape's matrices on the device (and their merged transpose, built there), proving RelaxedR1CSSNARK
     from a running instance (W, u, X), E in one C-ABI call.  mats: [(row_ptr, col, val bytes canonical)] over z = (W, u, X), as
-    RelaxedR1CSProver takes them."""
+    RelaxedR1CSProver takes them.  verifier_only=True (or SpartanContext.verifier) keeps the matrices alone, without the prover's
+    transpose: it verifies, evaluates the matrices and checks recursive proofs (recursive.recursive_verify) as a full context does, and
+    the library refuses to prove with it."""
 
-    def __init__(self, field_id, mats, n_w, n_x):
-        self.field, self.n_w, self.n_x = field_id, n_w, n_x
+    def __init__(self, field_id, mats, n_w, n_x, verifier_only=False):
+        self.field, self.n_w, self.n_x, self.verifier_only = field_id, n_w, n_x, verifier_only
         self.p = int.from_bytes(field_modulus(field_id), "little")
         self.rows = len(mats[0][0]) - 1
         keep = []
@@ -520,12 +522,18 @@ class SpartanContext:
         arr = lambda k: (C.c_void_p * 3)(*[keep[3 * m + k].ctypes.data for m in range(3)])
         ctx = C.c_void_p()
         self._ctx = None
-        _capi.check(_capi.lib().lurk_spartan_ctx_create(field_id, n_w, n_x, self.rows, arr(0), arr(1), arr(2), _capi.FMT_CANONICAL, C.byref(ctx)))
+        create = _capi.lib().lurk_spartan_ctx_create_verifier if verifier_only else _capi.lib().lurk_spartan_ctx_create
+        _capi.check(create(field_id, n_w, n_x, self.rows, arr(0), arr(1), arr(2), _capi.FMT_CANONICAL, C.byref(ctx)))
         self._ctx = ctx
         lr, lv, jl = C.c_int(), C.c_int(), C.c_size_t()
         _capi.check(_capi.lib().lurk_spartan_ctx_info(ctx, None, C.byref(lr), C.byref(lv), C.byref(jl)))
         self.log_rows, self.log_vars, self.joint_len = lr.value, lv.value, jl.value
         self.num_vars = 1 << self.log_vars
+
+    @classmethod
+    def verifier(cls, field_id, mats, n_w, n_x):
+        """a verifier-only context (lurk_spartan_ctx_create_verifier)"""
+        return cls(field_id, mats, n_w, n_x, verifier_only=True)
 
     def close(self):
         if self._ctx:
