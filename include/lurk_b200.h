@@ -494,6 +494,72 @@ int lurk_compress_prove_dev(lurk_compress_ctx *ctx, int n_primary, const void *c
                             const uint8_t *const *comm_E, const void *d_z2, const void *d_E2, const uint8_t comm_W2[96], const uint8_t comm_E2[96],
                             lurk_compress_challenge_fn challenge, void *user, int flags, lurk_compress_proof *out, int fmt, void *stream);
 
+/* Compressed verifier: CompressedSNARK::verify (Nova's Proof::verify on a compressed proof, src/proof/nova.rs:358-373; SuperNova's,
+ * supernova.rs:304-317) in one call, for the proof lurk_compress_prove_dev writes.  Per circuit, in order:
+ *   1. RelaxedR1CSSNARK::verify (BatchedRelaxedR1CSSNARK::verify with LURK_COMPRESS_BATCHED) up to the opening, as lurk_spartan_verify /
+ *      _batch run it (sum-checks, claims, batch_eval_reduce's verifier);
+ *   2. the joint commitment sum_i weights_i C_i over [comm_W_0 .., comm_E_0 ..] on the host;
+ *   3. the opening of the joint polynomial at r with value joint_eval:
+ *      IPA       round 0 comm | joint_eval -> the scale of ck_c; eq(r) in stream-ordered scratch; InnerProductArgument::verify as
+ *                lurk_ipa_verify_dev runs it, its rounds numbered 1 .. m;
+ *      HyperKZG  round 0 com -> r; the fold consistency 2 r Y[i+1] = r (1 - x) (v0[i] + v1[i]) + x (v0[i] - v1[i]), x = point[m - 1 - i],
+ *                Y = v[2] | joint_eval; round 1 v -> q; round 2 w -> d; then, with B = sum_j q^j com_j (com_0 = the joint commitment),
+ *                u = (r, -r, r^2) and B(u_t) = sum_j q^j v[t][j], the two G1 points
+ *                    P = sum_t d^t (B - B(u_t) G + u_t w_t),   Q = sum_t d^t w_t
+ *                and the caller's pairing check e(P, H) == e(Q, beta H).  Under a key of known beta it holds exactly when P == beta Q.
+ * The pairing stays with the caller, as the transcript does: `pairing` gets the circuit and P, Q (96 bytes each, `fmt`, the header's form),
+ * writes *holds (0 or 1) and returns 0, or non-zero to abort.
+ *
+ * Not here, as in lurk_compress_prove_dev: the secondary's NIFS::verify, which folds l_u_secondary into r_U_secondary with the RO challenge.
+ * u2, X2, comm_W2 and comm_E2 are f_U_secondary's, already folded by the caller; the RO hashes, the transcript, serde and the pairing too.
+ *
+ * The transcript is lurk_compress_challenge_fn with the calls of lurk_compress_prove_dev, in the same order, with the same messages: one
+ * transcript object serves prover and verifier.  HyperKZG's round 2 returns the verifier's d (the prover ignores it).  For one circuit the
+ * callbacks (transcript and pairing) come in protocol order and never concurrently with themselves; the two circuits' may run at once.
+ *
+ * The primary runs on the calling thread and `stream`, the secondary on a library-owned thread and a stream forked from `stream`; both are
+ * joined before the call returns, errors included.  LURK_COMPRESS_SEQUENTIAL runs the secondary after the primary, on the calling thread and
+ * `stream`.  Synchronous.
+ *
+ * Contexts: primary (n_primary, distinct) and secondary Spartan contexts, full or verifier-only, give the same results.  The IPA key contexts
+ * are borrowed: they must have no launch pending and must not be used by the caller during the call (as lurk_recursive_verify).
+ *
+ * Inputs, `fmt`: u (n_primary x 32), X[i] (n_x_i x 32), comm_W[i] / comm_E[i] (96) of the primary instances; u2, X2, comm_W2, comm_E2 of the
+ * secondary's.  proof: read are snark.outer_rounds, claims, inner_rounds, eval_W, reduce_rounds, claims_left (round polynomials in
+ * `rounds_fmt`, LURK_SPARTAN_ROUNDS_*), and com, v, w (HyperKZG) or L, R, a_final (IPA); comm, b_final and the snark's derived fields are
+ * neither read nor written.
+ *
+ * Result: out[0] primary, out[1] secondary.  snark_ok: step 1; eval_ok: HyperKZG's fold consistency, 1 for IPA; opening_ok: the pairing
+ * callback's answer, or IPA's closing check.  1 = holds, 0 = fails, -1 = not reached: the first failing check ends that circuit, and the other
+ * circuit is unaffected.  *accepted = 1 when all six hold.  A rejected proof is LURK_OK with *accepted = 0.
+ * Errors, all raised before the first callback and before any device work: values >= p and points off the curve (u, X, the commitments, every
+ * proof field read, g, ck_c) are LURK_ERR_RANGE; null pointers, n_primary out of range or not matching the contexts, mixed fields, a
+ * secondary field that is not the cycle partner, a key that is too short, on the wrong curve, on another device or with a launch pending, a
+ * context passed twice, HyperKZG without `pairing` are LURK_ERR_ARG.  A failing transcript or pairing callback is LURK_ERR_ARG with a message
+ * naming the circuit, never a rejection.  After an error the verdicts read -1 where not reached. */
+typedef struct lurk_compress_vk_pcs {
+    int kind;              /* LURK_PCS_HYPERKZG | LURK_PCS_IPA                                                              */
+    lurk_msm_ctx *ck;      /* IPA: the Pedersen key, >= joint_len bases, not consumed;  HyperKZG: NULL                      */
+    const uint8_t *ck_c;   /* IPA: 64 bytes affine, unscaled, `fmt`;  HyperKZG: NULL                                        */
+    const uint8_t *g;      /* HyperKZG: the verifier key's G1 point G (the key's first base), 64 bytes affine, `fmt`;  IPA: NULL */
+} lurk_compress_vk_pcs;
+/* e(P, H) == e(Q, beta H) under the caller's verifier key?  Writes *holds (0 / 1) and returns 0, or non-zero to abort. */
+typedef int (*lurk_pairing_check_fn)(void *user, int circuit, const uint8_t P[96], const uint8_t Q[96], int *holds);
+typedef struct lurk_compress_verdict {
+    int snark_ok;     /* RelaxedR1CSSNARK / BatchedRelaxedR1CSSNARK::verify up to the opening                 */
+    int eval_ok;      /* HyperKZG: the fold consistency of v;  IPA: 1;                  -1 = not reached      */
+    int opening_ok;   /* HyperKZG: the pairing callback's answer;  IPA: the closing check;  -1 = not reached  */
+} lurk_compress_verdict;
+int lurk_compress_verify(int n_primary, lurk_spartan_ctx *const *primary, lurk_spartan_ctx *secondary, const lurk_compress_vk_pcs *pcs_primary,
+                         const lurk_compress_vk_pcs *pcs_secondary, const uint8_t *u, const uint8_t *const *X, const uint8_t *const *comm_W,
+                         const uint8_t *const *comm_E, const uint8_t u2[32], const uint8_t *X2, const uint8_t comm_W2[96], const uint8_t comm_E2[96],
+                         const lurk_compress_proof *proof, int rounds_fmt, lurk_compress_challenge_fn challenge, lurk_pairing_check_fn pairing,
+                         void *user, int flags, lurk_compress_verdict out[2], int *accepted, int fmt, void *stream);
+/* sum_k scalars[k] points[k] on the host (Straus, split over host threads): the point arithmetic of the compressed verifier -- the joint
+ * commitment, HyperKZG's P and Q -- for callers that compose the verifier themselves.  points: count x 96 bytes of the header's form, scalars:
+ * count x 32 bytes, out: 96 bytes, all `fmt`.  Host only; works without a GPU. */
+int lurk_point_combination(int curve_id, const uint8_t *points_xyz, const uint8_t *scalars, size_t count, int fmt, uint8_t out_xyz[96]);
+
 /* ---------------------------------------------------------------------------------------------------
  * S5  Fold helpers on device-resident vectors (Arecibo NIFS::prove / R1CSShape::commit_T /
  *     RelaxedR1CSWitness::fold; SURVEY.md Appendix B).  All vectors Montgomery form on the device.

@@ -60,6 +60,16 @@ pub struct lurk_compress_proof { pub primary: lurk_compress_circuit_proof, pub s
 /// primary, 1 = secondary; the two circuits' calls may come from two threads at once (one transcript per circuit).
 pub type lurk_compress_challenge_fn = unsafe extern "C" fn(user: *mut c_void, circuit: c_int, phase: c_int, round: c_int, message: *const u8,
                                                            message_len: usize, challenge_out: *mut u8) -> c_int;
+/// the compressed verifier's evaluation engine (include/lurk_b200.h: lurk_compress_vk_pcs): IPA ck + ck_c (unscaled), HyperKZG g (the key's G1
+/// base); the other pointers null
+#[repr(C)]
+pub struct lurk_compress_vk_pcs { pub kind: c_int, pub ck: *mut lurk_msm_ctx, pub ck_c: *const u8, pub g: *const u8 }
+/// `int (*)(void *user, int circuit, const uint8_t P[96], const uint8_t Q[96], int *holds)`: e(P, H) == e(Q, beta H) under the verifier key
+pub type lurk_pairing_check_fn = unsafe extern "C" fn(user: *mut c_void, circuit: c_int, p: *const u8, q: *const u8, holds: *mut c_int) -> c_int;
+/// one circuit's verdict: 1 holds, 0 fails, -1 not reached
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct lurk_compress_verdict { pub snark_ok: c_int, pub eval_ok: c_int, pub opening_ok: c_int }
 /// one instance of RecursiveSNARK::verify's is_sat checks (include/lurk_b200.h: lurk_recursive_instance); e / comm_e null for a strict
 /// instance (l_u_secondary)
 #[repr(C)]
@@ -187,6 +197,14 @@ extern "C" {
                                    comm_w: *const *const u8, comm_e: *const *const u8, d_z2: *const c_void, d_e2: *const c_void, comm_w2: *const u8,
                                    comm_e2: *const u8, challenge: lurk_compress_challenge_fn, user: *mut c_void, flags: c_int,
                                    out: *mut lurk_compress_proof, fmt: c_int, stream: *mut c_void) -> c_int;
+    // N4 -- CompressedSNARK::verify (src/proof/nova.rs:358-373): after NIFS::verify of the secondary, which stays in Rust
+    pub fn lurk_compress_verify(n_primary: c_int, primary: *const *mut lurk_spartan_ctx, secondary: *mut lurk_spartan_ctx,
+                                pcs_primary: *const lurk_compress_vk_pcs, pcs_secondary: *const lurk_compress_vk_pcs, u: *const u8,
+                                x: *const *const u8, comm_w: *const *const u8, comm_e: *const *const u8, u2: *const u8, x2: *const u8,
+                                comm_w2: *const u8, comm_e2: *const u8, proof: *const lurk_compress_proof, rounds_fmt: c_int,
+                                challenge: lurk_compress_challenge_fn, pairing: Option<lurk_pairing_check_fn>, user: *mut c_void, flags: c_int,
+                                out: *mut lurk_compress_verdict, accepted: *mut c_int, fmt: c_int, stream: *mut c_void) -> c_int;
+    pub fn lurk_point_combination(curve_id: c_int, points_xyz: *const u8, scalars: *const u8, count: usize, fmt: c_int, out_xyz: *mut u8) -> c_int;
 }
 pub const LURK_SPARTAN_ROUNDS_EVALS: c_int = 0;
 pub const LURK_SPARTAN_ROUNDS_COMPRESSED: c_int = 1;
@@ -352,3 +370,36 @@ pub unsafe fn ipa_verify<F: FnMut(i32, &[u8]) -> Option<[u8; 32]>>(curve_id: c_i
     Ok(accepted != 0)
 }
 impl Drop for SpartanCtx { fn drop(&mut self) { unsafe { lurk_spartan_ctx_destroy(self.0) } } }
+
+/// CompressedSNARK::verify in one call.  `transcript(circuit, phase, round, msg)` is the prover's callback (one transcript per circuit; the two
+/// circuits may call at once, so it must be Sync), `pairing(P, Q)` the HyperKZG check e(P, H) == e(Q, beta H).  `inst` = (u, X, comm_W,
+/// comm_E) per primary instance, `inst2` = f_U_secondary's, already folded by NIFS::verify.  Returns (accepted, verdicts).
+/// # Safety: `proof`'s buffers have the sizes include/lurk_b200.h gives; X slices hold each shape's n_x elements.
+pub unsafe fn compress_verify<T, P>(primary: &[&SpartanCtx], secondary: &SpartanCtx, pcs: [&lurk_compress_vk_pcs; 2], u: &[u8], inst: &[(&[u8], &[u8; 96], &[u8; 96])],
+                                    inst2: (&[u8; 32], &[u8], &[u8; 96], &[u8; 96]), proof: &lurk_compress_proof, batched: bool, transcript: &T, pairing: &P)
+                                    -> Result<(bool, [lurk_compress_verdict; 2]), B200Error>
+where T: Fn(i32, i32, i32, &[u8]) -> Option<[u8; 32]> + Sync, P: Fn(i32, &[u8; 96], &[u8; 96]) -> Option<bool> + Sync {
+    struct User<'a, T, P> { t: &'a T, p: &'a P }
+    unsafe extern "C" fn tr<T: Fn(i32, i32, i32, &[u8]) -> Option<[u8; 32]> + Sync, P>(user: *mut c_void, circuit: c_int, phase: c_int, round: c_int,
+                                                                                     msg: *const u8, len: usize, out: *mut u8) -> c_int {
+        let u = &*(user as *const User<T, P>);
+        let m = if len == 0 { &[][..] } else { std::slice::from_raw_parts(msg, len) };
+        match (u.t)(circuit, phase, round, m) { Some(r) => { std::ptr::copy_nonoverlapping(r.as_ptr(), out, 32); 0 } None => 1 }
+    }
+    unsafe extern "C" fn pc<T, P: Fn(i32, &[u8; 96], &[u8; 96]) -> Option<bool> + Sync>(user: *mut c_void, circuit: c_int, p: *const u8, q: *const u8,
+                                                                                      holds: *mut c_int) -> c_int {
+        let u = &*(user as *const User<T, P>);
+        match (u.p)(circuit, &*(p as *const [u8; 96]), &*(q as *const [u8; 96])) { Some(h) => { *holds = h as c_int; 0 } None => 1 }
+    }
+    let user = User { t: transcript, p: pairing };
+    let raw: Vec<*mut lurk_spartan_ctx> = primary.iter().map(|c| c.0).collect();
+    let xs: Vec<*const u8> = inst.iter().map(|i| i.0.as_ptr()).collect();
+    let cw: Vec<*const u8> = inst.iter().map(|i| i.1.as_ptr()).collect();
+    let ce: Vec<*const u8> = inst.iter().map(|i| i.2.as_ptr()).collect();
+    let (mut out, mut accepted) = ([lurk_compress_verdict::default(); 2], 0 as c_int);
+    check(lurk_compress_verify(raw.len() as c_int, raw.as_ptr(), secondary.0, pcs[0], pcs[1], u.as_ptr(), xs.as_ptr(), cw.as_ptr(), ce.as_ptr(),
+                               inst2.0.as_ptr(), inst2.1.as_ptr(), inst2.2.as_ptr(), inst2.3.as_ptr(), proof, LURK_SPARTAN_ROUNDS_COMPRESSED, tr::<T, P>,
+                               Some(pc::<T, P>), &user as *const User<T, P> as *mut c_void, if batched { LURK_COMPRESS_BATCHED } else { 0 },
+                               out.as_mut_ptr(), &mut accepted, LURK_FMT_MONTGOMERY, std::ptr::null_mut()))?;
+    Ok((accepted != 0, out))
+}

@@ -8,7 +8,7 @@ commitment key); it never computes on the CPU -- every call goes to the CUDA lib
 from . import _capi, compress, recursive, spartan
 from ._capi import (CURVE_BN254_G1, CURVE_GRUMPKIN, CURVE_PALLAS, CURVE_VESTA, FIELD_BN254_FQ, FIELD_BN254_FR,
                     FIELD_PALLAS_FP, FIELD_PALLAS_FQ, FMT_CANONICAL, FMT_MONTGOMERY, LurkError)
-from .compress import CompressContext, compress_prove
+from .compress import CompressContext, compress_prove, compress_verify
 from .recursive import recursive_verify
 from .commit import (CommitmentKey, ShardedCommitmentKey, ck_size, from_label, hash_to_curve_batch, point_sum, shake256, shard_bounds,
                      synthetic_bases)
@@ -20,7 +20,7 @@ from .trie import StandardTrie, Trie
 
 __all__ = [
     "CommitmentKey", "ShardedCommitmentKey", "NovaFoldContext", "SuperNovaFoldContext", "point_sum", "shard_bounds", "synthetic_bases", "ck_size", "from_label",
-    "compress", "CompressContext", "compress_prove", "recursive", "recursive_verify",
+    "compress", "CompressContext", "compress_prove", "compress_verify", "recursive", "recursive_verify",
     "hash_to_curve_batch", "shake256", "spartan", "HashConstants", "PoseidonCache", "SlotType",
     "compute_witness_size", "generate_slots_witnesses", "slot_witness_batch_bytes", "StoreCore", "StandardTrie", "Trie", "LurkError",
     "FIELD_BN254_FR", "FIELD_BN254_FQ", "FIELD_PALLAS_FQ", "FIELD_PALLAS_FP", "CURVE_BN254_G1", "CURVE_GRUMPKIN",

@@ -81,6 +81,19 @@ class CompressProof(C.Structure):
     _fields_ = [("primary", CompressCircuitProof), ("secondary", CompressCircuitProof)]
 
 
+# the compressed verifier (lurk_compress_verify)
+class CompressVkPcs(C.Structure):
+    _fields_ = [("kind", C.c_int), ("ck", C.c_void_p), ("ck_c", C.c_void_p), ("g", C.c_void_p)]
+
+
+class CompressVerdict(C.Structure):
+    _fields_ = [("snark_ok", C.c_int), ("eval_ok", C.c_int), ("opening_ok", C.c_int)]
+
+
+# lurk_pairing_check_fn: int (*)(void *user, int circuit, const uint8_t P[96], const uint8_t Q[96], int *holds)
+PAIRING_CHECK_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_uint8), C.POINTER(C.c_uint8), C.POINTER(C.c_int))
+
+
 # the recursive verifier (lurk_recursive_verify, _dev)
 class RecursiveInstance(C.Structure):
     _fields_ = [(name, C.c_void_p) for name in ("shape", "ck", "z", "E", "comm_W", "comm_E")]
@@ -159,6 +172,10 @@ PROTOTYPES = {
     "lurk_compress_ctx_info": (_i, [_vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "lurk_compress_prove_dev": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp), _vp, _vp, _vp, _vp, COMPRESS_CHALLENGE_FN, _vp, _i,
                                      C.POINTER(CompressProof), _i, _vp]),
+    "lurk_compress_verify": (_i, [_i, C.POINTER(_vp), _vp, C.POINTER(CompressVkPcs), C.POINTER(CompressVkPcs), _vp, C.POINTER(_vp), C.POINTER(_vp),
+                                  C.POINTER(_vp), _vp, _vp, _vp, _vp, C.POINTER(CompressProof), _i, COMPRESS_CHALLENGE_FN, PAIRING_CHECK_FN, _vp, _i,
+                                  C.POINTER(CompressVerdict), C.POINTER(_i), _i, _vp]),
+    "lurk_point_combination": (_i, [_i, _vp, _vp, _sz, _i, _vp]),
     "lurk_recursive_verify_dev": (_i, [_i, C.POINTER(RecursiveInstance), C.POINTER(RecursiveVerdict), C.POINTER(_i), _i, _vp]),
     "lurk_recursive_verify": (_i, [_i, C.POINTER(RecursiveInstance), C.POINTER(RecursiveVerdict), C.POINTER(_i), _i, _vp]),
     "lurk_ipa_verify_dev": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, CHALLENGE_FN, _vp, C.POINTER(_i), _vp, _vp, _i, _vp]),

@@ -1,7 +1,8 @@
 """CompressedSNARK::prove (reference src/proof/nova.rs:341-356, supernova.rs:293-317) through the compress context of the C ABI
 (lurk_compress_ctx_*, lurk_compress_prove_dev; include/lurk_b200.h): for the primary and the secondary circuit, RelaxedR1CSSNARK::prove (or
 SuperNova's BatchedRelaxedR1CSSNARK::prove), batch_eval_reduce, the joint commitment and the opening of the joint polynomial -- HyperKZG or
-the inner-product argument -- in one call, the two circuits proved at once on library-owned threads and streams.
+the inner-product argument -- in one call, the two circuits proved at once on library-owned threads and streams.  CompressedSNARK::verify
+(nova.rs:358-373, supernova.rs:304-317) through lurk_compress_verify: the same transcript, the pairing of HyperKZG left to a callback.
 
 The transcript is the caller's: challenge(circuit, label, data) -> int, circuit 0 = primary, 1 = secondary.  The Spartan phases use the labels
 and data of spartan.SpartanContext ("tau", "outer_r", "outer", "inner_r", "inner", "batch_eval"); the opening's calls are ("pcs", (round,
@@ -28,6 +29,30 @@ def _points(buf, k):
         b = buf[96 * i:96 * i + 96].tobytes()
         out.append((int.from_bytes(b[:32], "little"), int.from_bytes(b[32:64], "little")) if int.from_bytes(b[64:], "little") else None)
     return out
+
+
+def _transcript(challenge, circuits, native, errors):
+    """(lurk_compress_challenge_fn, user) for challenge(circuit, label, data), or native's; circuits: [(Spartan contexts, batched)] of the
+    primary and the secondary.  Exceptions of `challenge` go to `errors` and abort the call."""
+    if native:
+        return (native[0] if isinstance(native[0], _capi.COMPRESS_CHALLENGE_FN) else _capi.COMPRESS_CHALLENGE_FN(native[0])), native[1]
+    ps = [ctxs[0].p for ctxs, _ in circuits]
+
+    def cb(user, circuit, phase, rnd, msg, msg_len, out):
+        try:
+            ctxs, bat = circuits[circuit]
+            data = C.string_at(msg, msg_len) if msg_len else b""
+            if phase == _capi.SPARTAN_PCS:
+                x = challenge(circuit, "pcs", (rnd, data))
+            else:
+                x = challenge(circuit, *_spartan_label(phase, rnd, data, len(ctxs), bat))
+            for i, byte in enumerate((int(x) % ps[circuit]).to_bytes(32, "little")):
+                out[i] = byte
+            return 0
+        except Exception as e:          # never unwind through the C frames
+            errors.append(e)
+            return 1
+    return _capi.COMPRESS_CHALLENGE_FN(cb), None
 
 
 class CompressContext:
@@ -102,27 +127,7 @@ class CompressContext:
         cw = (C.c_void_p * n)(*[p.ctypes.data for p in pts[:n]])
         ce = (C.c_void_p * n)(*[p.ctypes.data for p in pts[n:2 * n]])
         errors = []
-        ps = [ctxs[0].p for ctxs, _, _ in circuits]
-
-        def cb(user, circuit, phase, rnd, msg, msg_len, out):
-            try:
-                ctxs, bat, _ = circuits[circuit]
-                data = C.string_at(msg, msg_len) if msg_len else b""
-                if phase == _capi.SPARTAN_PCS:
-                    x = challenge(circuit, "pcs", (rnd, data))
-                else:
-                    x = challenge(circuit, *_spartan_label(phase, rnd, data, len(ctxs), bat))
-                for i, byte in enumerate((int(x) % ps[circuit]).to_bytes(32, "little")):
-                    out[i] = byte
-                return 0
-            except Exception as e:          # never unwind through the C frames
-                errors.append(e)
-                return 1
-        if native:
-            fn = native[0] if isinstance(native[0], _capi.COMPRESS_CHALLENGE_FN) else _capi.COMPRESS_CHALLENGE_FN(native[0])
-            user = native[1]
-        else:
-            fn, user = _capi.COMPRESS_CHALLENGE_FN(cb), None
+        fn, user = _transcript(challenge, [(ctxs, bat) for ctxs, bat, _ in circuits], native, errors)
         flags = (_capi.COMPRESS_SEQUENTIAL if sequential else 0) | (_capi.COMPRESS_BATCHED if batched else 0)
         rc = _capi.lib().lurk_compress_prove_dev(self._ctx, n, ptr_arr([x[0] for x in primary]), ptr_arr([x[1] for x in primary]), cw, ce,
                                                  C.c_void_p(secondary[0]), C.c_void_p(secondary[1]), C.c_void_p(pts[2 * n].ctypes.data),
@@ -157,3 +162,81 @@ def compress_prove(ctx, primary, secondary, challenge, **kw):
     """CompressContext.prove as a function"""
     return ctx.prove(primary, secondary, challenge, **kw)
 
+
+
+def _flat(rounds):
+    return _fes([x for rnd in rounds for x in rnd])
+
+
+def _point_list(pts):
+    return np.concatenate([_point(P) for P in pts]) if pts else np.zeros(96, dtype=np.uint8)
+
+
+def compress_verify(primary, secondary, pcs_primary, pcs_secondary, instances, instance2, proof, challenge, pairing=None, batched=None,
+                    sequential=False, compressed=False, stream=0, native=None, native_pairing=None):
+    """CompressedSNARK::verify through lurk_compress_verify.  primary: a SpartanContext (Nova) or a list of them (SuperNova), secondary: a
+    SpartanContext; full or verifier-only.  pcs_primary / pcs_secondary: ("hyperkzg", g) with g the KZG key's first base as (x, y), or ("ipa",
+    CommitmentKey, ck_c as (x, y), unscaled).  instances: [(u, X, comm_W, comm_E)] per primary context; instance2: the secondary's (u, X,
+    comm_W, comm_E) of f_U_secondary, the last fold already made.  proof: [primary, secondary] as compress_prove returns them (with
+    compressed=True their round polynomials as CompressedUniPoly: every coefficient but the linear one).  challenge(circuit, label, data) ->
+    int as for compress_prove; pairing(circuit, P, Q) -> bool, P and Q as (x, y) or None, answers e(P, H) == e(Q, beta H).  native /
+    native_pairing: (a C function or its address, user pointer) and a C function or its address, called instead of `challenge` / `pairing`.
+    Returns (accepted, [(snark_ok, eval_ok, opening_ok) of the primary, of the secondary]), -1 for a check not reached."""
+    ctxs = list(primary) if isinstance(primary, (list, tuple)) else [primary]
+    n = len(ctxs)
+    assert len(instances) == n
+    batched = n > 1 if batched is None else batched
+    circuits = [(ctxs, batched), ([secondary], False)]
+    kinds = [pcs_primary[0], pcs_secondary[0]]
+    keep, rec, vk = [], _capi.CompressProof(), []
+    for k, (pr, spec) in enumerate(zip(proof, (pcs_primary, pcs_secondary))):
+        bat = circuits[k][1]
+        claims = pr["claims"] if bat else [pr["claims"]]
+        eval_W = pr["eval_W"] if bat else [pr["eval_W"]]
+        b = dict(outer_rounds=_flat(pr["outer_rounds"]), claims=_flat(claims), inner_rounds=_flat(pr["inner_rounds"]), eval_W=_fes(eval_W),
+                 reduce_rounds=_flat(pr["reduce_rounds"]), claims_left=_fes(pr["claims_left"]))
+        if spec[0] == "hyperkzg":
+            o = dict(com=_point_list(pr["com"]), v=_flat(pr["v"]), w=_point_list(pr["w"]))
+            g = _fes([spec[1][0], spec[1][1]])
+            vk.append(_capi.CompressVkPcs(_capi.PCS_HYPERKZG, None, None, g.ctypes.data))
+        else:
+            o = dict(L=_point_list(pr["L"]), R=_point_list(pr["R"]), a_final=_fes([pr["a_final"]]))
+            g = _fes([spec[2][0], spec[2][1]])
+            vk.append(_capi.CompressVkPcs(_capi.PCS_IPA, spec[1]._ctx, g.ctypes.data, None))
+        keep += [b, o, g]
+        cp = rec.primary if k == 0 else rec.secondary
+        cp.snark = _capi.SpartanProof(**{key: v.ctypes.data for key, v in b.items()})
+        for key, v in o.items():
+            setattr(cp, key, v.ctypes.data)
+    us = _fes([x[0] for x in instances])
+    xs = [_fes(x[1]) for x in instances] + [_fes(instance2[1])]
+    pts = [_point(x[2]) for x in instances] + [_point(x[3]) for x in instances] + [_point(instance2[2]), _point(instance2[3])]
+    u2 = _fes([instance2[0]])
+    arr = lambda vals: (C.c_void_p * n)(*[C.c_void_p(v) for v in vals])
+    errors = []
+    fn, user = _transcript(challenge, circuits, native, errors)
+
+    def pcb(user, circuit, P, Q, holds):
+        try:
+            pq = _points(np.ctypeslib.as_array(P, (96,)), 1) + _points(np.ctypeslib.as_array(Q, (96,)), 1)
+            holds[0] = 1 if pairing(circuit, *pq) else 0
+            return 0
+        except Exception as e:          # never unwind through the C frames
+            errors.append(e)
+            return 1
+    if native_pairing:
+        pfn = native_pairing if isinstance(native_pairing, _capi.PAIRING_CHECK_FN) else _capi.PAIRING_CHECK_FN(native_pairing)
+    else:
+        pfn = _capi.PAIRING_CHECK_FN(pcb) if pairing else _capi.PAIRING_CHECK_FN()
+    flags = (_capi.COMPRESS_SEQUENTIAL if sequential else 0) | (_capi.COMPRESS_BATCHED if batched else 0)
+    verdicts, acc = (_capi.CompressVerdict * 2)(), C.c_int(-1)
+    rc = _capi.lib().lurk_compress_verify(n, arr([c._ctx.value for c in ctxs]), secondary._ctx, C.byref(vk[0]), C.byref(vk[1]), C.c_void_p(us.ctypes.data),
+                                          arr([x.ctypes.data for x in xs[:n]]), arr([p.ctypes.data for p in pts[:n]]),
+                                          arr([p.ctypes.data for p in pts[n:2 * n]]), C.c_void_p(u2.ctypes.data), C.c_void_p(xs[n].ctypes.data),
+                                          C.c_void_p(pts[2 * n].ctypes.data), C.c_void_p(pts[2 * n + 1].ctypes.data), C.byref(rec),
+                                          _capi.SPARTAN_ROUNDS_COMPRESSED if compressed else _capi.SPARTAN_ROUNDS_EVALS, fn, pfn, user, flags, verdicts,
+                                          C.byref(acc), _capi.FMT_CANONICAL, C.c_void_p(stream))
+    if errors:
+        raise errors[0]
+    _capi.check(rc)
+    return bool(acc.value), [(v.snark_ok, v.eval_ok, v.opening_ok) for v in verdicts]

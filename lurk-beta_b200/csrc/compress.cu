@@ -8,13 +8,10 @@
 #include "common.cuh"
 #include "pcs.cuh"
 #include "sc_scratch.cuh"
+#include "worker.cuh"
 
 #include <algorithm>
-#include <condition_variable>
-#include <functional>
-#include <mutex>
 #include <string>
-#include <thread>
 #include <vector>
 
 namespace lurk {
@@ -24,45 +21,6 @@ int spartan_prove_checked(int n, lurk_spartan_ctx *const *ctxs, const void *cons
 int refuse_verifier_only(const lurk_spartan_ctx *ctx, const char *who);                                       // spartan.cu
 
 constexpr int CP_MAX_PRIMARY = 30;
-
-// One host thread running one job at a time, for as long as the context lives.
-class Worker {
-  public:
-    Worker() : th_([this] { loop(); }) {}
-    ~Worker() {
-        { std::lock_guard<std::mutex> g(mu_); stop_ = true; }
-        cv_.notify_all();
-        th_.join();
-    }
-    void post(std::function<void()> f) {
-        { std::lock_guard<std::mutex> g(mu_); job_ = std::move(f); }
-        cv_.notify_all();
-    }
-    void wait() {
-        std::unique_lock<std::mutex> g(mu_);
-        cv_.wait(g, [&] { return !job_; });
-    }
-
-  private:
-    void loop() {
-        std::unique_lock<std::mutex> g(mu_);
-        for (;;) {
-            cv_.wait(g, [&] { return stop_ || job_; });
-            if (!job_) return;
-            std::function<void()> f = job_;
-            g.unlock();
-            f();
-            g.lock();
-            job_ = nullptr;
-            cv_.notify_all();
-        }
-    }
-    std::mutex mu_;
-    std::condition_variable cv_;
-    std::function<void()> job_;
-    bool stop_ = false;
-    std::thread th_;            // last: the thread starts once the members it uses exist
-};
 
 struct Circuit {
     std::vector<lurk_spartan_ctx *> sp;

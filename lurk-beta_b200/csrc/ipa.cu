@@ -368,6 +368,14 @@ int ipa_prove_arena(int curve_id, lurk_msm_ctx *ck, PcsArena &a, const uint8_t *
     });
 }
 
+int ipa_verify_checked(int curve_id, lurk_msm_ctx *ck, const uint8_t *gc_bytes, const uint8_t *comm, const uint8_t *c, const void *d_b, int log_n,
+                       const uint8_t *L, const uint8_t *R, const uint8_t *a_final, lurk_challenge_fn challenge, void *user, int *accepted, int fmt,
+                       cudaStream_t s) {
+    return dispatch_curve(curve_id, [&](auto cv) {
+        return ipa_verify<decltype(cv)>(ck, gc_bytes, comm, c, d_b, log_n, L, R, a_final, challenge, user, accepted, nullptr, nullptr, fmt, s);
+    });
+}
+
 template <class C>
 static typename C::Base curve_b() {
     const Affine<typename C::Base> g = curve_generator<C>();

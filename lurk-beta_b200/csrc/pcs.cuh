@@ -39,6 +39,10 @@ int hyperkzg_prove_arena(int curve_id, lurk_msm_ctx *ck, PcsArena &a, const void
 // InnerProductArgument::prove's rounds on the arena; d_a / d_b consumed as by lurk_ipa_prove_dev
 int ipa_prove_arena(int curve_id, lurk_msm_ctx *ck, PcsArena &a, const uint8_t *gc_bytes, void *d_a, void *d_b, int log_n, lurk_challenge_fn challenge,
                     void *user, uint8_t *L_out, uint8_t *R_out, uint8_t *a_final, uint8_t *b_final, int fmt, cudaStream_t s);
+// InnerProductArgument::verify as lurk_ipa_verify_dev runs it, for a caller that has checked the key (curve, >= 2^log_n bases) and the pointers
+int ipa_verify_checked(int curve_id, lurk_msm_ctx *ck, const uint8_t *gc_bytes, const uint8_t *comm, const uint8_t *c, const void *d_b, int log_n,
+                       const uint8_t *L, const uint8_t *R, const uint8_t *a_final, lurk_challenge_fn challenge, void *user, int *accepted, int fmt,
+                       cudaStream_t s);
 // every 96-byte point x | y | z of the header's form (z = 1 on the curve, or the identity 0 | 0 | 0), in `fmt`; host only
 bool points_valid(int curve_id, const uint8_t *const *points, int count, int fmt);
 // an affine point x | y (identity = (0, 0)) of the curve, in `fmt`; host only

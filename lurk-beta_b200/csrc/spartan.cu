@@ -650,6 +650,44 @@ static int sumcheck_verify(const uint8_t *rounds_in, int rounds, int deg, int ro
     return LURK_OK;
 }
 
+// The verifier's inputs read and range-checked: u, X of every instance and the proof's fields.  A value >= p is an error, not a rejection.
+template <class F>
+static int verify_inputs(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u_in, const uint8_t *const *X_in, const lurk_spartan_proof *proof,
+                         int rounds_fmt, int fmt, std::vector<F> &u, std::vector<std::vector<F>> &X, std::vector<F> &cl, std::vector<F> &ew,
+                         std::vector<F> &left) {
+    int maxS = 0, maxT = 0;
+    for (int i = 0; i < n; i++) {
+        maxS = std::max(maxS, ctxs[i]->log_rows);
+        maxT = std::max(maxT, ctxs[i]->log_vars + 1);
+    }
+    const int m = std::max(maxS, maxT - 1);
+    const bool evals = rounds_fmt == LURK_SPARTAN_ROUNDS_EVALS;
+    const int fid = ctxs[0]->field_id;
+    u.assign(n, F::zero());
+    cl.assign(4 * (size_t)n, F::zero());
+    ew.assign(n, F::zero());
+    left.assign(2 * (size_t)n, F::zero());
+    X.assign(n, {});
+    for (int i = 0; i < n; i++) {
+        if (!fe_in(u_in + 32 * i, fmt, u[i])) { set_error("u of instance %d is not reduced", i); return LURK_ERR_RANGE; }
+        X[i].resize(ctxs[i]->n_x);
+        for (uint64_t k = 0; k < ctxs[i]->n_x; k++)
+            if (!fe_in(X_in[i] + 32 * k, fmt, X[i][k])) { set_error("X[%llu] of instance %d is not reduced", (unsigned long long)k, i); return LURK_ERR_RANGE; }
+    }
+    struct Field { const uint8_t *p; size_t count; const char *name; F *out; };
+    const Field fields[] = {{proof->outer_rounds, (size_t)maxS * (evals ? 4 : 3), "outer_rounds", nullptr},
+                            {proof->inner_rounds, (size_t)maxT * (evals ? 3 : 2), "inner_rounds", nullptr},
+                            {proof->reduce_rounds, (size_t)m * (evals ? 3 : 2), "reduce_rounds", nullptr},
+                            {proof->claims, 4 * (size_t)n, "claims", cl.data()},
+                            {proof->eval_W, (size_t)n, "eval_W", ew.data()},
+                            {proof->claims_left, 2 * (size_t)n, "claims_left", left.data()}};
+    for (const Field &f : fields) {
+        if (!all_reduced(f.p, f.count, fmt, fid)) { set_error("proof field %s holds a value that is not reduced", f.name); return LURK_ERR_RANGE; }
+        for (size_t k = 0; f.out && k < f.count; k++) fe_in(f.p + 32 * k, fmt, f.out[k]);
+    }
+    return LURK_OK;
+}
+
 // RelaxedR1CSSNARK::verify (batched = false, n = 1) or BatchedRelaxedR1CSSNARK::verify up to the opening, then the verifier of
 // batch_eval_reduce over [W_i .., E_i ..]: the same transcript calls as spartan_prove, in the same order.  The matrices' evaluations at
 // (rx_i, ry_i) are one sp_matrix_eval_kernel launch per instance and one synchronisation; everything else is O(log) host arithmetic (and
@@ -669,28 +707,10 @@ static int spartan_verify(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u
         maxT = std::max(maxT, T[i]);
     }
     const int m = std::max(maxS, maxT - 1);
-    const bool evals = rounds_fmt == LURK_SPARTAN_ROUNDS_EVALS;
-    // every input is checked before the first transcript call: a value >= p is an error, not a rejection
-    const int fid = ctxs[0]->field_id;
-    std::vector<F> u(n), cl(4 * (size_t)n), ew(n), left(2 * (size_t)n);
-    std::vector<std::vector<F>> X(n);
-    for (int i = 0; i < n; i++) {
-        if (!fe_in(u_in + 32 * i, fmt, u[i])) { set_error("u of instance %d is not reduced", i); return LURK_ERR_RANGE; }
-        X[i].resize(C[i]->n_x);
-        for (uint64_t k = 0; k < C[i]->n_x; k++)
-            if (!fe_in(X_in[i] + 32 * k, fmt, X[i][k])) { set_error("X[%llu] of instance %d is not reduced", (unsigned long long)k, i); return LURK_ERR_RANGE; }
-    }
-    struct Field { const uint8_t *p; size_t count; const char *name; F *out; };
-    const Field fields[] = {{proof->outer_rounds, (size_t)maxS * (evals ? 4 : 3), "outer_rounds", nullptr},
-                            {proof->inner_rounds, (size_t)maxT * (evals ? 3 : 2), "inner_rounds", nullptr},
-                            {proof->reduce_rounds, (size_t)m * (evals ? 3 : 2), "reduce_rounds", nullptr},
-                            {proof->claims, 4 * (size_t)n, "claims", cl.data()},
-                            {proof->eval_W, (size_t)n, "eval_W", ew.data()},
-                            {proof->claims_left, 2 * (size_t)n, "claims_left", left.data()}};
-    for (const Field &f : fields) {
-        if (!all_reduced(f.p, f.count, fmt, fid)) { set_error("proof field %s holds a value that is not reduced", f.name); return LURK_ERR_RANGE; }
-        for (size_t k = 0; f.out && k < f.count; k++) fe_in(f.p + 32 * k, fmt, f.out[k]);
-    }
+    // every input is checked before the first transcript call
+    std::vector<F> u, cl, ew, left;
+    std::vector<std::vector<F>> X;
+    LURK_TRY(verify_inputs<F>(n, ctxs, u_in, X_in, proof, rounds_fmt, fmt, u, X, cl, ew, left));
 
     // tau, outer_r
     std::vector<std::vector<F>> tau(n);
@@ -881,6 +901,31 @@ static int check_verify_args(int n, lurk_spartan_ctx *const *ctxs, const uint8_t
     }
     return LURK_OK;
 }
+
+namespace lurk {
+
+// every check lurk_spartan_verify / _batch make before their first transcript call -- the arguments, then the values of u, X and the proof
+// -- for compress_verify.cu, which makes them for both circuits before either circuit's transcript starts
+int spartan_verify_precheck(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u, const uint8_t *const *X, const lurk_spartan_proof *proof,
+                            int rounds_fmt, lurk_spartan_challenge_fn fn, const int *accepted, int fmt) {
+    LURK_TRY(check_verify_args(n, ctxs, u, X, proof, rounds_fmt, fn, accepted, fmt));
+    return dispatch_field(ctxs[0]->field_id, [&](auto f) {
+        using F = decltype(f);
+        std::vector<F> uv, cl, ew, left;
+        std::vector<std::vector<F>> Xv;
+        return verify_inputs<F>(n, ctxs, u, X, proof, rounds_fmt, fmt, uv, Xv, cl, ew, left);
+    });
+}
+
+// the verifier behind lurk_spartan_verify / _batch for compress_verify.cu, after spartan_verify_precheck
+int spartan_verify_checked(int n, lurk_spartan_ctx *const *ctxs, const uint8_t *u, const uint8_t *const *X, lurk_spartan_proof *proof, int rounds_fmt,
+                           lurk_spartan_challenge_fn fn, void *user, int *accepted, int fmt, cudaStream_t s, bool batched) {
+    return dispatch_field(ctxs[0]->field_id, [&](auto f) {
+        return spartan_verify<decltype(f)>(n, ctxs, u, X, proof, rounds_fmt, fn, user, accepted, fmt, s, batched);
+    });
+}
+
+}  // namespace lurk
 
 static int spartan_ctx_create(int field_id, uint64_t n_w, uint64_t n_x, uint64_t n_rows, const uint64_t *const row_ptr[3], const uint32_t *const col[3],
                               const uint8_t *const val[3], int fmt, bool verifier_only, lurk_spartan_ctx **out) {
