@@ -157,6 +157,10 @@ int lurk_msm_ctx_run_dev(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int
  * window (c = 20) becomes affordable: ~13 instead of 16 bucket additions per scalar.  Results are unchanged.
  * Call before cloning; clones share the table. */
 int lurk_msm_ctx_precompute(lurk_msm_ctx *ctx);
+/* The same with a chosen window width c (10 .. 22: at most 26 windows) instead of the one the key's size suggests: the fold context builds its own tables
+ * with c = 16, where one bucket set (2^15 counters) fits a CTA's shared memory and the digit sort keeps its histogram on chip.
+ * LURK_ERR_ARG when the context already has a table. */
+int lurk_msm_ctx_precompute_window(lurk_msm_ctx *ctx, int c);
 /* Asynchronous form: `launch` enqueues the whole commitment on `stream` and returns; `finish` waits for it and
  * produces the point.  One launch may be pending per context; `clone` gives another context on the same resident key
  * (own scratch; the parent must outlive it) so that e.g. commit(W) and commit(T) of one fold overlap. */
@@ -167,6 +171,8 @@ int lurk_msm_ctx_clone(lurk_msm_ctx *ctx, lurk_msm_ctx **out);
  * kernel) on the launching stream; last_profile returns its duration and the number of kernels the run launched. */
 int lurk_msm_ctx_set_profiling(lurk_msm_ctx *ctx, int enable);
 int lurk_msm_ctx_last_profile(lurk_msm_ctx *ctx, float *accumulate_ms, unsigned *kernel_launches);
+/* with profiling enabled: device time of the last finished run's digit sort (first memset to the end of the scatter kernel) */
+int lurk_msm_ctx_last_sort_ms(lurk_msm_ctx *ctx, float *sort_ms);
 /* one-shot convenience (uploads bases every call) */
 int lurk_msm(int curve_id, const uint8_t *bases_affine, const uint8_t *scalars, size_t n, int fmt,
              uint8_t out_xyz[96]);

@@ -133,8 +133,10 @@ PROTOTYPES = {
     "lurk_msm_ctx_finish": (_i, [_vp, _vp]),
     "lurk_msm_ctx_clone": (_i, [_vp, C.POINTER(_vp)]),
     "lurk_msm_ctx_precompute": (_i, [_vp]),
+    "lurk_msm_ctx_precompute_window": (_i, [_vp, _i]),
     "lurk_msm_ctx_set_profiling": (_i, [_vp, _i]),
     "lurk_msm_ctx_last_profile": (_i, [_vp, C.POINTER(C.c_float), C.POINTER(C.c_uint)]),
+    "lurk_msm_ctx_last_sort_ms": (_i, [_vp, C.POINTER(C.c_float)]),
     "lurk_point_sum": (_i, [_i, _vp, _sz, _i, _vp]),
     "lurk_synthetic_bases": (_i, [_i, C.c_uint64, _sz, _i, _vp]),
     "lurk_ck_size": (_sz, [_sz, _sz, _sz]),

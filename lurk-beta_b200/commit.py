@@ -81,9 +81,13 @@ class CommitmentKey:
         _capi.check(_capi.lib().lurk_msm_ctx_finish(self._ctx, _capi.np_ptr(out)))
         return out
 
-    def precompute(self):
-        """build the fixed-base window table on the device (once per key; call before clone())"""
-        _capi.check(_capi.lib().lurk_msm_ctx_precompute(self._ctx))
+    def precompute(self, window=0):
+        """build the fixed-base window table on the device (once per key; call before clone()); window: width in bits instead of the
+        one the key's size suggests (at 16 or less the digit sort keeps its histogram in shared memory)"""
+        if window:
+            _capi.check(_capi.lib().lurk_msm_ctx_precompute_window(self._ctx, window))
+        else:
+            _capi.check(_capi.lib().lurk_msm_ctx_precompute(self._ctx))
         return self
 
     def clone(self):
@@ -102,6 +106,12 @@ class CommitmentKey:
         ms, k = C.c_float(), C.c_uint()
         _capi.check(_capi.lib().lurk_msm_ctx_last_profile(self._ctx, C.byref(ms), C.byref(k)))
         return ms.value, k.value
+
+    def last_sort_ms(self):
+        """device ms of the last run's digit sort (profiling enabled)"""
+        ms = C.c_float()
+        _capi.check(_capi.lib().lurk_msm_ctx_last_sort_ms(self._ctx, C.byref(ms)))
+        return ms.value
 
     def close(self):
         if getattr(self, "_ctx", None) and self._ctx.value:

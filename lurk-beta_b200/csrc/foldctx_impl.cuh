@@ -29,8 +29,9 @@ static constexpr int FOLD_MAX_SPANS = 4;
 static constexpr int FOLD_RO_RATE = 24;            // Arecibo's RO: neptune sponge over PoseidonConstants<_, U24>
 // Windows of the fold's own tables.  On an H100 (400 W) at fib rc = 100, W = 16 / 17 / 18 and T = 15 / 16 / 17 all land within
 // 1 % of each other (4.31-4.37 ms per fold, about the run-to-run spread); a narrower window than the key's c = 20 shortens the
-// bucket reduction on the chain.
-static constexpr int FOLD_W_WINDOW = 17;           // window of commit(W2 - D) (own table when narrower than the key's)
+// bucket reduction on the chain.  At 16 bits or less one bucket set (2^15 counters) fits a CTA's shared memory and the digit sort
+// keeps its histogram there (msm_hist_smem_kernel); W = 17 would keep the global-atomics sort for commit(W2 - D).
+static constexpr int FOLD_W_WINDOW = 16;           // window of commit(W2 - D) (own table when narrower than the key's)
 static constexpr int FOLD_T_WINDOW = 16;           // widest window of the chain-critical commit(T)
 
 // ----------------------------------------------------------------------------- fold kernels (witness field)

@@ -44,6 +44,7 @@ int lurk_msm_ctx_set_profiling(lurk_msm_ctx *ctx, int enable) {
     if (enable && !ctx->ev0) {
         LURK_CUDA_TRY(cudaEventCreate(&ctx->ev0));
         LURK_CUDA_TRY(cudaEventCreate(&ctx->ev1));
+        LURK_CUDA_TRY(cudaEventCreate(&ctx->ev_sort));
     }
     ctx->profile = enable != 0;
     return LURK_OK;
@@ -52,6 +53,15 @@ int lurk_msm_ctx_last_profile(lurk_msm_ctx *ctx, float *accumulate_ms, unsigned 
     if (!ctx) { set_error("null context"); return LURK_ERR_ARG; }
     if (accumulate_ms) *accumulate_ms = ctx->last_accumulate_ms;
     if (kernel_launches) *kernel_launches = ctx->last_launches;
+    return LURK_OK;
+}
+
+int lurk_msm_ctx_last_sort_ms(lurk_msm_ctx *ctx, float *sort_ms) {
+    if (!ctx || !sort_ms) { set_error("null argument"); return LURK_ERR_ARG; }
+    std::lock_guard<std::mutex> g(ctx->mu);
+    *sort_ms = 0.f;
+    if (ctx->pending) { set_error("a launch is pending on this context"); return LURK_ERR_ARG; }
+    if (ctx->ev_sort) LURK_CUDA_TRY(cudaEventElapsedTime(sort_ms, ctx->ev_sort, ctx->ev0));
     return LURK_OK;
 }
 
@@ -65,6 +75,7 @@ int lurk_msm_ctx_info(lurk_msm_ctx *ctx, int *curve_id, size_t *n) {
 void lurk_msm_ctx_destroy(lurk_msm_ctx *ctx) {
     if (!ctx) return;
     if (ctx->ev0) { cudaEventDestroy(ctx->ev0); cudaEventDestroy(ctx->ev1); }
+    if (ctx->ev_sort) cudaEventDestroy(ctx->ev_sort);
     if (ctx->done) cudaEventDestroy(ctx->done);
     if (ctx->ev_fork) { cudaEventDestroy(ctx->ev_fork); cudaEventDestroy(ctx->ev_join); }
     if (ctx->owns_bases && ctx->d_bases) cudaFree(ctx->d_bases);
@@ -98,6 +109,16 @@ int lurk_msm_ctx_precompute(lurk_msm_ctx *ctx) {
     if (ctx->d_table || ctx->n == 0) return LURK_OK;
     if (ctx->pending) { set_error("a launch is pending on this context"); return LURK_ERR_ARG; }
     return dispatch_curve(ctx->curve_id, [&](auto cv) { return msm_precompute<decltype(cv)>(ctx, 0); });
+}
+
+int lurk_msm_ctx_precompute_window(lurk_msm_ctx *ctx, int c) {
+    if (!ctx) { set_error("null context"); return LURK_ERR_ARG; }
+    std::lock_guard<std::mutex> g(ctx->mu);
+    if (ctx->d_table) { set_error("the context already has a fixed-base table"); return LURK_ERR_ARG; }
+    if (ctx->n == 0) return LURK_OK;
+    if (ctx->pending) { set_error("a launch is pending on this context"); return LURK_ERR_ARG; }
+    if (c <= 0) { set_error("window width %d out of range", c); return LURK_ERR_ARG; }
+    return dispatch_curve(ctx->curve_id, [&](auto cv) { return msm_precompute<decltype(cv)>(ctx, c); });
 }
 
 int lurk_msm_ctx_clone(lurk_msm_ctx *ctx, lurk_msm_ctx **out) {

@@ -10,6 +10,8 @@
 //   1. digits+histogram: one thread per scalar; signed c-bit windows (buckets 1..2^(c-1), sign folded into the point);
 //      warp-aggregated atomics (__match_any_sync) so the 0/1-heavy witness vectors (SURVEY.md H6) do not serialise on
 //      one counter.
+//      Fixed-base mode with c <= 16 keeps the histogram (and in step 3 the cursors) in shared memory, one private copy per CTA:
+//      msm_hist_smem_kernel / msm_hist_columns_kernel / msm_scatter_smem_kernel below.
 //   2. exclusive scan of the (windows x 2^(c-1)) bucket counts.
 //   3. scatter: point index | sign written at its bucket's next slot (counting sort; order inside a bucket is free
 //      because point addition commutes -- the affine result is canonical).
@@ -230,6 +232,92 @@ __global__ void __launch_bounds__(256) msm_scatter_kernel(const Fs *__restrict__
         if (key != KEY_NONE) {
             uint32_t rank = __popc(peers & ((1u << lane) - 1));
             sorted[offsets[key] + base + rank] = ((uint32_t)i + (uint32_t)w * base_stride) | (neg << 31);
+        }
+    }
+}
+
+// ---- the same counting sort with the histogram and the cursors in shared memory (fixed-base mode, c <= 16) ----------------------
+// All windows of the fixed-base mode share ONE bucket set, so the whole histogram is nb * 4 bytes: 128 KB at c = 16, inside the
+// 227 KB a CTA may have on sm_90.  A persistent grid of G CTAs (one per SM) gives each CTA a contiguous range of scalars and a
+// private histogram; the digits of a full-width scalar are spread over 2^15 buckets, where the warp aggregation of the kernels
+// above merges nothing and every digit costs a global atomic in each pass.  Here a zero scalar (two thirds of the fold's vectors)
+// costs one load and no window walk: nothing needs converged lanes.
+//   msm_hist_smem_kernel     cnt[g][b] = digits of CTA g's range in bucket b
+//   msm_hist_columns_kernel  cnt[g][b] -> exclusive prefix over g; counts[b] = column total (the scan kernels above take it from there)
+//   msm_scatter_smem_kernel  cursor[b] = offsets[b] + cnt[g][b] in shared memory: the CTAs' ranges inside a bucket are disjoint
+static constexpr uint32_t MSM_SORT_THREADS = 1024;
+static constexpr size_t MSM_SORT_SMEM_MAX = (size_t)128 << 10;
+
+// scalar i as the sort sees it (minus the constant part, canonical); false when it is zero and contributes no digit
+template <class Fs>
+__device__ __forceinline__ bool sort_scalar(const Fs *__restrict__ scalars, const Fs *__restrict__ sub, size_t i, int fmt, Fs &k) {
+    k = load_fe<Fs>(scalars + i);
+    if (sub) k = k - load_fe<Fs>(sub + i);
+    if (k.is_zero()) return false;               // zero is zero in either form
+    if (fmt == LURK_FMT_MONTGOMERY) k = k.to_canonical();
+    return true;
+}
+
+template <class Fs>
+__global__ void __launch_bounds__(MSM_SORT_THREADS) msm_hist_smem_kernel(const Fs *__restrict__ scalars, const Fs *__restrict__ sub, size_t n, int fmt, int c,
+                                                                         int nwin, uint32_t nb, uint32_t *__restrict__ cnt) {
+    extern __shared__ uint32_t sort_smem[];
+    for (uint32_t b = threadIdx.x; b < nb; b += MSM_SORT_THREADS) sort_smem[b] = 0;
+    __syncthreads();
+    const size_t lo = (size_t)blockIdx.x * n / gridDim.x, hi = (size_t)(blockIdx.x + 1) * n / gridDim.x;
+    const uint32_t half = 1u << (c - 1);
+    for (size_t i = lo + threadIdx.x; i < hi; i += MSM_SORT_THREADS) {
+        Fs k;
+        if (!sort_scalar(scalars, sub, i, fmt, k)) continue;
+        uint32_t carry = 0;
+        for (int w = 0; w < nwin; w++) {
+            const uint32_t raw = window_bits(k.v, w * c, c) + carry;
+            carry = raw > half;
+            const uint32_t mag = carry ? (1u << c) - raw : raw;
+            if (mag) atomicAdd(sort_smem + (mag - 1), 1u);
+        }
+    }
+    __syncthreads();
+    uint32_t *row = cnt + (size_t)blockIdx.x * nb;
+    for (uint32_t b = threadIdx.x; b < nb; b += MSM_SORT_THREADS) row[b] = sort_smem[b];
+}
+
+static __global__ void __launch_bounds__(256) msm_hist_columns_kernel(uint32_t *__restrict__ cnt, uint32_t G, uint32_t nb, uint32_t *__restrict__ counts) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    uint32_t run = 0;
+    for (uint32_t g0 = 0; g0 < G; g0 += 8) {     // eight independent loads in flight per thread
+        uint32_t v[8];
+#pragma unroll
+        for (uint32_t j = 0; j < 8; j++) v[j] = g0 + j < G ? cnt[(size_t)(g0 + j) * nb + b] : 0u;
+#pragma unroll
+        for (uint32_t j = 0; j < 8; j++) {
+            if (g0 + j < G) cnt[(size_t)(g0 + j) * nb + b] = run;
+            run += v[j];
+        }
+    }
+    counts[b] = run;
+}
+
+template <class Fs>
+__global__ void __launch_bounds__(MSM_SORT_THREADS) msm_scatter_smem_kernel(const Fs *__restrict__ scalars, const Fs *__restrict__ sub, size_t n, int fmt, int c,
+                                                                            int nwin, uint32_t nb, uint32_t base_stride, const uint32_t *__restrict__ offsets,
+                                                                            const uint32_t *__restrict__ cnt, uint32_t *__restrict__ sorted) {
+    extern __shared__ uint32_t sort_smem[];
+    const uint32_t *row = cnt + (size_t)blockIdx.x * nb;
+    for (uint32_t b = threadIdx.x; b < nb; b += MSM_SORT_THREADS) sort_smem[b] = offsets[b] + row[b];
+    __syncthreads();
+    const size_t lo = (size_t)blockIdx.x * n / gridDim.x, hi = (size_t)(blockIdx.x + 1) * n / gridDim.x;
+    const uint32_t half = 1u << (c - 1);
+    for (size_t i = lo + threadIdx.x; i < hi; i += MSM_SORT_THREADS) {
+        Fs k;
+        if (!sort_scalar(scalars, sub, i, fmt, k)) continue;
+        uint32_t carry = 0;
+        for (int w = 0; w < nwin; w++) {
+            const uint32_t raw = window_bits(k.v, w * c, c) + carry;
+            carry = raw > half;
+            const uint32_t mag = carry ? (1u << c) - raw : raw;
+            if (mag) sorted[atomicAdd(sort_smem + (mag - 1), 1u)] = ((uint32_t)i + (uint32_t)w * base_stride) | (carry << 31);
         }
     }
 }
@@ -662,7 +750,7 @@ __global__ void __launch_bounds__(256) msm_bases_to_mont_kernel(Fb *coords, size
 
 // ----------------------------------------------------------------------------- context
 struct MsmScratch {
-    DevBuf counts, offsets, tiles, sorted, buckets, ppt, chunks, chunk_sums, slices, wins, result, scalars, pair_offs[2], pair_pts[2];
+    DevBuf counts, hist, offsets, tiles, sorted, buckets, ppt, chunks, chunk_sums, slices, wins, result, scalars, pair_offs[2], pair_pts[2];
     void *h_wins = nullptr;   // pinned
     void *h_stage[2] = {nullptr, nullptr};          // pinned staging for host-buffer scalars
     cudaEvent_t stage_done[2] = {nullptr, nullptr};
@@ -691,7 +779,7 @@ struct lurk_msm_ctx {
     MsmScratch scratch;
     // optional device timing of the dominant kernel (bucket accumulation), on the launching stream
     bool profile = false;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_sort = nullptr;   // ev_sort .. ev0: the digit sort; ev0 .. ev1: the accumulation
     float last_accumulate_ms = 0.f;
     unsigned last_launches = 0;
     // launch / finish split
@@ -780,10 +868,16 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     const uint32_t t1_alloc = std::max(t1, P.t1);
     // a long bucket holds more than MSM_LONG_PARTIALS segment starts, so there are at most t1 / (MSM_LONG_PARTIALS + 1)
     const uint32_t max_long = t1 / (MSM_LONG_PARTIALS + 1) + 1;
+    // digit sort: per-CTA shared-memory histograms when one bucket set fits a CTA's shared memory (see msm_hist_smem_kernel).
+    // LURK_MSM_SORT=legacy forces the global-atomics kernels (tuning aid, read at every launch so that one process can compare both)
+    const char *sort_env = getenv("LURK_MSM_SORT");
+    const bool smem_sort = fixed && (size_t)P.nb * sizeof(uint32_t) <= MSM_SORT_SMEM_MAX && !(sort_env && !strcmp(sort_env, "legacy"));
+    const uint32_t sort_ctas = (uint32_t)std::min<size_t>((size_t)sm_count(), (n + MSM_SORT_THREADS - 1) / MSM_SORT_THREADS);
     {
         // scratch grows monotonically; a context is normally run at one size (the circuit's witness length)
         auto ensure = [](DevBuf &b, size_t bytes) { return b.bytes >= bytes ? LURK_OK : b.alloc(bytes); };
         LURK_TRY(ensure(S.counts, (((size_t)TB + 1) * 2 + 1 + max_long) * sizeof(uint32_t)));   // counts | cursor | long count | long list
+        if (smem_sort) LURK_TRY(ensure(S.hist, (size_t)sort_ctas * P.nb * sizeof(uint32_t)));   // cnt[G][nb]
         LURK_TRY(ensure(S.offsets, ((size_t)TB + 1) * sizeof(uint32_t)));
         LURK_TRY(ensure(S.tiles, ((size_t)ntiles + 1) * 2 * sizeof(uint32_t)));  // tile sums | tile offsets
         LURK_TRY(ensure(S.sorted, n * (size_t)P.nwin * sizeof(uint32_t)));
@@ -805,19 +899,36 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     uint32_t *long_list = cursor + (TB + 1) + 1;                        // long_list[-1] is zeroed with the counts
     Pt *buckets = S.buckets.as<Pt>();       // every bucket is written by the accumulation or the merge: no clearing
 
-    LURK_CUDA_TRY(cudaMemsetAsync(counts, 0, (((size_t)TB + 1) * 2 + 1) * sizeof(uint32_t), s));
-    const unsigned gs = (unsigned)((n + 255) / 256);
+    if (ctx->profile) LURK_CUDA_TRY(cudaEventRecord(ctx->ev_sort, s));
     unsigned launches = 0;
     const uint32_t key_stride = fixed ? 0u : P.nb;                 // fixed-base: all windows share one bucket set
     const uint32_t base_stride = fixed ? (uint32_t)ctx->n : 0u;     // ... and address table[w * n + i]
     const Affine<Fb> *bases = (const Affine<Fb> *)(fixed ? ctx->d_table : ctx->d_bases);
     const Fs *sub = (!readback && fmt == LURK_FMT_MONTGOMERY) ? (const Fs *)ctx->d_sub : nullptr;
-    msm_count_kernel<Fs><<<gs, 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, counts);
+    if (smem_sort) {
+        const size_t smem = (size_t)P.nb * sizeof(uint32_t);
+        uint32_t *cnt = S.hist.as<uint32_t>();
+        if (smem > ((size_t)48 << 10)) {   // above the default limit a kernel opts in, per device
+            LURK_CUDA_TRY(cudaFuncSetAttribute(msm_hist_smem_kernel<Fs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            LURK_CUDA_TRY(cudaFuncSetAttribute(msm_scatter_smem_kernel<Fs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        }
+        LURK_CUDA_TRY(cudaMemsetAsync(long_list - 1, 0, sizeof(uint32_t), s));     // every count is written: only the long-list length is cleared
+        msm_hist_smem_kernel<Fs><<<sort_ctas, MSM_SORT_THREADS, smem, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, P.nb, cnt);
+        msm_hist_columns_kernel<<<(P.nb + 255) / 256, 256, 0, s>>>(cnt, sort_ctas, P.nb, counts);
+        launches++;
+    } else {
+        LURK_CUDA_TRY(cudaMemsetAsync(counts, 0, (((size_t)TB + 1) * 2 + 1) * sizeof(uint32_t), s));
+        msm_count_kernel<Fs><<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, counts);
+    }
     msm_scan_tile_sums_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_sums);
     msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
     // the offsets the accumulation walks also give the merge its long buckets (after the last pair round, if any)
     msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, rounds ? nullptr : long_list);
-    msm_scatter_kernel<Fs><<<gs, 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, base_stride, offsets, cursor, sorted);
+    if (smem_sort)
+        msm_scatter_smem_kernel<Fs><<<sort_ctas, MSM_SORT_THREADS, (size_t)P.nb * sizeof(uint32_t), s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, P.nb, base_stride,
+                                                                                                       offsets, S.hist.as<uint32_t>(), sorted);
+    else
+        msm_scatter_kernel<Fs><<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, base_stride, offsets, cursor, sorted);
     if (ctx->profile) LURK_CUDA_TRY(cudaEventRecord(ctx->ev0, s));
     // ---- pair rounds
     const uint32_t *acc_offs = offsets;

@@ -120,7 +120,7 @@ def main():
         for e in wk:
             if not e["name"].startswith("void lurk::msm_"):
                 break
-            if "msm_count_kernel" in e["name"]:
+            if "msm_count_kernel" in e["name"] or "msm_hist_smem_kernel" in e["name"]:   # the next commitment's sort
                 break
             tailk.append(e)
         if tailk:
