@@ -44,7 +44,7 @@ def chal_fn(p, log):
     return f
 
 
-@pytest.mark.parametrize("curve", [0, 2])
+@pytest.mark.parametrize("curve", [0, 1, 2, 3])
 def test_powers_of_tau_match_oracle(L, spec, curve):
     Cv = spec.CURVES[curve]
     pb, q = spec.FIELD_MODULUS[Cv["base"]], spec.FIELD_MODULUS[Cv["scalar"]]
