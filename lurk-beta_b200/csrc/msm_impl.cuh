@@ -10,8 +10,8 @@
 //   1. digits+histogram: one thread per scalar; signed c-bit windows (buckets 1..2^(c-1), sign folded into the point);
 //      warp-aggregated atomics (__match_any_sync) so the 0/1-heavy witness vectors (SURVEY.md H6) do not serialise on
 //      one counter.
-//      Fixed-base mode with c <= 16 keeps the histogram (and in step 3 the cursors) in shared memory, one private copy per CTA:
-//      msm_hist_smem_kernel / msm_hist_columns_kernel / msm_scatter_smem_kernel below.
+//      Fixed-base mode with c <= 16 keeps the histogram in shared memory, one private copy per CTA, and replaces step 3 by two
+//      coalesced passes (by bucket range, then by bucket): msm_hist_smem_kernel .. msm_range_sort_kernel below.
 //   2. exclusive scan of the (windows x 2^(c-1)) bucket counts.
 //   3. scatter: point index | sign written at its bucket's next slot (counting sort; order inside a bucket is free
 //      because point addition commutes -- the affine result is canonical).
@@ -236,19 +236,42 @@ __global__ void __launch_bounds__(256) msm_scatter_kernel(const Fs *__restrict__
     }
 }
 
-// ---- the same counting sort with the histogram and the cursors in shared memory (fixed-base mode, c <= 16) ----------------------
+// ---- the same counting sort in two coalesced levels (fixed-base mode, c <= 16) ----------------------------------------------------
 // All windows of the fixed-base mode share ONE bucket set, so the whole histogram is nb * 4 bytes: 128 KB at c = 16, inside the
 // 227 KB a CTA may have on sm_90.  A persistent grid of G CTAs (one per SM) gives each CTA a contiguous range of scalars and a
 // private histogram; the digits of a full-width scalar are spread over 2^15 buckets, where the warp aggregation of the kernels
-// above merges nothing and every digit costs a global atomic in each pass.  Here a zero scalar (two thirds of the fold's vectors)
-// costs one load and no window walk: nothing needs converged lanes.
-//   msm_hist_smem_kernel     cnt[g][b] = digits of CTA g's range in bucket b
-//   msm_hist_columns_kernel  cnt[g][b] -> exclusive prefix over g; counts[b] = column total (the scan kernels above take it from there)
-//   msm_scatter_smem_kernel  cursor[b] = offsets[b] + cnt[g][b] in shared memory: the CTAs' ranges inside a bucket are disjoint
+// above merges nothing.  Here a zero scalar (two thirds of the fold's vectors) costs one load and no window walk.
+// Writing each digit straight to its bucket's slot is one scattered 4-byte store per digit (a CTA holds ~1.4 digits per bucket at
+// c = 16, too few to stage); instead the buckets are grouped into ranges of MSM_RANGE_BUCKETS consecutive buckets and the digits
+// move in two coalesced passes, first to their range, then inside it to their bucket:
+//   msm_hist_smem_kernel     cnt[g][b] = digits of CTA g's scalars in bucket b; rng[g][j] = the same per range j
+//   msm_hist_columns_kernel  counts[b] = column total of cnt, tile sums of counts for the scan; rng[g][j] -> exclusive prefix over g
+//   (the scan kernels above turn counts into offsets)
+//   msm_partition_kernel     CTA g re-walks its scalars a tile at a time, groups the tile's digits by range in shared memory and
+//                            appends each group to the CTA's slice of the range's span [offsets[first bucket], offsets[last + 1])
+//                            as 8-byte entries (sorted word, bucket): runs of dozens of entries instead of single words
+//   msm_range_sort_kernel    fixed-size slices of every range's span: a counting sort by bucket in shared memory, then each bucket's
+//                            run is written out contiguously at a place taken from a per-bucket cursor (one global atomic per bucket
+//                            and slice, so a hot bucket spread over many slices -- a 0/1-heavy witness -- still spreads over all SMs)
 static constexpr uint32_t MSM_SORT_THREADS = 1024;
 static constexpr size_t MSM_SORT_SMEM_MAX = (size_t)128 << 10;
+static constexpr uint32_t MSM_RANGE_BITS = 7, MSM_RANGE_BUCKETS = 1u << MSM_RANGE_BITS;   // 256 ranges at c = 16
+static constexpr uint32_t MSM_MAX_RANGES = (1u << 15) / MSM_RANGE_BUCKETS;
+static constexpr uint32_t MSM_PART_DIGITS = 32768;      // digits a partition tile stages (6 B each: 192 KB)
+static constexpr uint32_t MSM_PART_SCALARS = 2 * MSM_SORT_THREADS;
+static constexpr uint32_t MSM_RSORT_PER_THREAD = 8, MSM_RSORT_SLICE = MSM_RSORT_PER_THREAD * MSM_SORT_THREADS;
+
+__host__ __device__ __forceinline__ uint32_t msm_ranges(uint32_t nb) { return (nb + MSM_RANGE_BUCKETS - 1) / MSM_RANGE_BUCKETS; }
+// scalars per partition tile: every digit of the tile fits the staging buffer
+inline uint32_t msm_part_scalars(int nwin) { return std::min<uint32_t>(MSM_PART_SCALARS, MSM_PART_DIGITS / (uint32_t)nwin); }
 
 // scalar i as the sort sees it (minus the constant part, canonical); false when it is zero and contributes no digit
+template <class Fs>
+__device__ __forceinline__ void prefetch_scalar(const Fs *__restrict__ scalars, const Fs *__restrict__ sub, size_t i) {
+    // the sort kernels run one 1024-thread CTA per SM with a serial chain per thread: ask L2 for the next scalar early
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(scalars + i));
+    if (sub) asm volatile("prefetch.global.L2 [%0];" ::"l"(sub + i));
+}
 template <class Fs>
 __device__ __forceinline__ bool sort_scalar(const Fs *__restrict__ scalars, const Fs *__restrict__ sub, size_t i, int fmt, Fs &k) {
     k = load_fe<Fs>(scalars + i);
@@ -258,67 +281,218 @@ __device__ __forceinline__ bool sort_scalar(const Fs *__restrict__ scalars, cons
     return true;
 }
 
+// f(w, bucket, negative) for every non-zero signed digit of k.  The fold tables' shape (c = 16, 16 windows) is unrolled at compile
+// time, so the window indices are constants and the scalar's limbs stay in registers instead of a stack frame indexed per window.
+template <int C, int NWIN, class Fs, class F>
+__device__ __forceinline__ void walk_digits_unrolled(const Fs &k, F f) {
+    uint32_t carry = 0;
+#pragma unroll
+    for (int w = 0; w < NWIN; w++) {
+        const uint32_t raw = window_bits(k.v, w * C, C) + carry;
+        carry = raw > (1u << (C - 1));
+        const uint32_t mag = carry ? (1u << C) - raw : raw;
+        if (mag) f((uint32_t)w, mag - 1, carry);
+    }
+}
+template <class Fs, class F>
+__device__ __forceinline__ void walk_digits(const Fs &k, int c, int nwin, F f) {
+    if (c == 16 && nwin == 16) { walk_digits_unrolled<16, 16>(k, f); return; }
+    uint32_t kv[8];                                  // a copy for the per-window indexing, so that k itself stays in registers
+#pragma unroll
+    for (int i = 0; i < 8; i++) kv[i] = k.v[i];
+    const uint32_t half = 1u << (c - 1);
+    uint32_t carry = 0;
+    for (int w = 0; w < nwin; w++) {
+        const uint32_t raw = window_bits(kv, w * c, c) + carry;
+        carry = raw > half;
+        const uint32_t mag = carry ? (1u << c) - raw : raw;
+        if (mag) f((uint32_t)w, mag - 1, carry);
+    }
+}
+
+// zero: `nzero` words the later kernels accumulate into (the scan's tile sums, the long-bucket count), cleared by CTA 0
 template <class Fs>
 __global__ void __launch_bounds__(MSM_SORT_THREADS) msm_hist_smem_kernel(const Fs *__restrict__ scalars, const Fs *__restrict__ sub, size_t n, int fmt, int c,
-                                                                         int nwin, uint32_t nb, uint32_t *__restrict__ cnt) {
+                                                                         int nwin, uint32_t nb, uint32_t *__restrict__ cnt, uint32_t *__restrict__ rng,
+                                                                         uint32_t *__restrict__ zero, uint32_t nzero) {
     extern __shared__ uint32_t sort_smem[];
+    if (blockIdx.x == 0)
+        for (uint32_t t = threadIdx.x; t < nzero; t += MSM_SORT_THREADS) zero[t] = 0;
     for (uint32_t b = threadIdx.x; b < nb; b += MSM_SORT_THREADS) sort_smem[b] = 0;
     __syncthreads();
     const size_t lo = (size_t)blockIdx.x * n / gridDim.x, hi = (size_t)(blockIdx.x + 1) * n / gridDim.x;
-    const uint32_t half = 1u << (c - 1);
     for (size_t i = lo + threadIdx.x; i < hi; i += MSM_SORT_THREADS) {
+        if (i + MSM_SORT_THREADS < hi) prefetch_scalar(scalars, sub, i + MSM_SORT_THREADS);
         Fs k;
         if (!sort_scalar(scalars, sub, i, fmt, k)) continue;
-        uint32_t carry = 0;
-        for (int w = 0; w < nwin; w++) {
-            const uint32_t raw = window_bits(k.v, w * c, c) + carry;
-            carry = raw > half;
-            const uint32_t mag = carry ? (1u << c) - raw : raw;
-            if (mag) atomicAdd(sort_smem + (mag - 1), 1u);
-        }
+        walk_digits(k, c, nwin, [&](uint32_t, uint32_t b, uint32_t) { atomicAdd(sort_smem + b, 1u); });
     }
     __syncthreads();
     uint32_t *row = cnt + (size_t)blockIdx.x * nb;
     for (uint32_t b = threadIdx.x; b < nb; b += MSM_SORT_THREADS) row[b] = sort_smem[b];
-}
-
-static __global__ void __launch_bounds__(256) msm_hist_columns_kernel(uint32_t *__restrict__ cnt, uint32_t G, uint32_t nb, uint32_t *__restrict__ counts) {
-    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= nb) return;
-    uint32_t run = 0;
-    for (uint32_t g0 = 0; g0 < G; g0 += 8) {     // eight independent loads in flight per thread
-        uint32_t v[8];
-#pragma unroll
-        for (uint32_t j = 0; j < 8; j++) v[j] = g0 + j < G ? cnt[(size_t)(g0 + j) * nb + b] : 0u;
-#pragma unroll
-        for (uint32_t j = 0; j < 8; j++) {
-            if (g0 + j < G) cnt[(size_t)(g0 + j) * nb + b] = run;
-            run += v[j];
-        }
+    // one warp per range
+    const uint32_t R = msm_ranges(nb), lane = threadIdx.x & 31;
+    for (uint32_t j = threadIdx.x >> 5; j < R; j += MSM_SORT_THREADS / 32) {
+        uint32_t v = 0;
+        for (uint32_t b = j * MSM_RANGE_BUCKETS + lane; b < min(nb, (j + 1) * MSM_RANGE_BUCKETS); b += 32) v += sort_smem[b];
+        v = __reduce_add_sync(0xffffffffu, v);
+        if (lane == 0) rng[(size_t)blockIdx.x * R + j] = v;
     }
-    counts[b] = run;
 }
 
-template <class Fs>
-__global__ void __launch_bounds__(MSM_SORT_THREADS) msm_scatter_smem_kernel(const Fs *__restrict__ scalars, const Fs *__restrict__ sub, size_t n, int fmt, int c,
-                                                                            int nwin, uint32_t nb, uint32_t base_stride, const uint32_t *__restrict__ offsets,
-                                                                            const uint32_t *__restrict__ cnt, uint32_t *__restrict__ sorted) {
-    extern __shared__ uint32_t sort_smem[];
-    const uint32_t *row = cnt + (size_t)blockIdx.x * nb;
-    for (uint32_t b = threadIdx.x; b < nb; b += MSM_SORT_THREADS) sort_smem[b] = offsets[b] + row[b];
-    __syncthreads();
-    const size_t lo = (size_t)blockIdx.x * n / gridDim.x, hi = (size_t)(blockIdx.x + 1) * n / gridDim.x;
-    const uint32_t half = 1u << (c - 1);
-    for (size_t i = lo + threadIdx.x; i < hi; i += MSM_SORT_THREADS) {
-        Fs k;
-        if (!sort_scalar(scalars, sub, i, fmt, k)) continue;
-        uint32_t carry = 0;
-        for (int w = 0; w < nwin; w++) {
-            const uint32_t raw = window_bits(k.v, w * c, c) + carry;
-            carry = raw > half;
-            const uint32_t mag = carry ? (1u << c) - raw : raw;
-            if (mag) sorted[atomicAdd(sort_smem + (mag - 1), 1u)] = ((uint32_t)i + (uint32_t)w * base_stride) | (carry << 31);
+// One thread per bucket: counts[b] = sum over the G rows, cursor[b] = 0 (msm_range_sort_kernel's), and each warp adds its buckets to
+// their scan tile's sum (tile_sums zeroed by msm_hist_smem_kernel) -- the first of the three scan launches, fused.  Warp j < R also
+// turns column j of rng into its exclusive prefix over the CTAs.
+static __global__ void __launch_bounds__(256) msm_hist_columns_kernel(const uint32_t *__restrict__ cnt, uint32_t *__restrict__ rng, uint32_t G, uint32_t nb,
+                                                                      uint32_t *__restrict__ counts, uint32_t *__restrict__ cursor,
+                                                                      uint32_t *__restrict__ tile_sums) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+    uint32_t run = 0;
+    if (b < nb) {
+        for (uint32_t g0 = 0; g0 < G; g0 += 8) {     // eight independent loads in flight per thread
+            uint32_t v[8];
+#pragma unroll
+            for (uint32_t j = 0; j < 8; j++) v[j] = g0 + j < G ? cnt[(size_t)(g0 + j) * nb + b] : 0u;
+#pragma unroll
+            for (uint32_t j = 0; j < 8; j++) run += v[j];
         }
+        counts[b] = run;
+        cursor[b] = 0;
+    }
+    const uint32_t wsum = __reduce_add_sync(0xffffffffu, run);
+    if (lane == 0 && wsum) atomicAdd(tile_sums + b / SCAN_TILE, wsum);     // a warp's 32 buckets lie in one tile
+    const uint32_t j = b >> 5, R = msm_ranges(nb);
+    if (j >= R) return;
+    uint32_t carry = 0;
+    for (uint32_t g0 = 0; g0 < G; g0 += 32) {
+        const uint32_t g = g0 + lane;
+        const uint32_t v = g < G ? rng[(size_t)g * R + j] : 0u;
+        uint32_t incl = v;
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= (uint32_t)d) incl += t; }
+        if (g < G) rng[(size_t)g * R + j] = carry + incl - v;
+        carry += __shfl_sync(0xffffffffu, incl, 31);
+    }
+}
+
+// CTA g: the scalars of msm_hist_smem_kernel's CTA g, `ts` at a time (two per thread; ts * nwin <= the staging buffer).  Per tile:
+// count the digits per range, scan, stage them grouped by range (sorted word + bucket, 6 B), then append each range's group to
+// the CTA's cursor in that range's span.  Consecutive threads write consecutive entries of one group: the stores coalesce.
+template <class Fs>
+__global__ void __launch_bounds__(MSM_SORT_THREADS) msm_partition_kernel(const Fs *__restrict__ scalars, const Fs *__restrict__ sub, size_t n, int fmt, int c,
+                                                                         int nwin, uint32_t nb, uint32_t ts, uint32_t base_stride,
+                                                                         const uint32_t *__restrict__ offsets, const uint32_t *__restrict__ rng,
+                                                                         uint2 *__restrict__ parts) {
+    extern __shared__ uint32_t part_smem[];
+    uint32_t *wbuf = part_smem;                                           // ts * nwin sorted words
+    uint16_t *bbuf = reinterpret_cast<uint16_t *>(part_smem + (size_t)ts * nwin);   // ... and their buckets
+    __shared__ uint32_t rcnt[MSM_MAX_RANGES], rstart[MSM_MAX_RANGES], rfill[MSM_MAX_RANGES], rcur[MSM_MAX_RANGES];
+    const uint32_t tid = threadIdx.x, R = msm_ranges(nb);
+    if (tid < R) rcur[tid] = offsets[tid * MSM_RANGE_BUCKETS] + rng[(size_t)blockIdx.x * R + tid];
+    const size_t lo = (size_t)blockIdx.x * n / gridDim.x, hi = (size_t)(blockIdx.x + 1) * n / gridDim.x;
+    for (size_t t0 = lo; t0 < hi; t0 += ts) {
+        if (tid < R) rcnt[tid] = 0;
+        __syncthreads();
+        Fs k[2];
+        bool live[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const uint32_t t = tid + h * MSM_SORT_THREADS;
+            if (t < ts && t0 + ts + t < hi) prefetch_scalar(scalars, sub, t0 + ts + t);      // the next tile's
+            live[h] = t < ts && t0 + t < hi && sort_scalar(scalars, sub, t0 + t, fmt, k[h]);
+            if (live[h]) walk_digits(k[h], c, nwin, [&](uint32_t, uint32_t b, uint32_t) { atomicAdd(rcnt + (b >> MSM_RANGE_BITS), 1u); });
+        }
+        __syncthreads();
+        uint32_t total;
+        const uint32_t ex = block_exclusive_scan_1024(tid < R ? rcnt[tid] : 0u, &total);
+        if (tid < R) { rstart[tid] = ex; rfill[tid] = ex; }
+        __syncthreads();
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            if (!live[h]) continue;
+            const uint32_t i = (uint32_t)(t0 + tid + h * MSM_SORT_THREADS);
+            walk_digits(k[h], c, nwin, [&](uint32_t w, uint32_t b, uint32_t neg) {
+                const uint32_t p = atomicAdd(rfill + (b >> MSM_RANGE_BITS), 1u);
+                wbuf[p] = (i + w * base_stride) | (neg << 31);
+                bbuf[p] = (uint16_t)b;
+            });
+        }
+        __syncthreads();
+        for (uint32_t p = tid; p < total; p += MSM_SORT_THREADS) {
+            const uint32_t b = bbuf[p], j = b >> MSM_RANGE_BITS;
+            parts[rcur[j] + p - rstart[j]] = make_uint2(wbuf[p], b);
+        }
+        __syncthreads();
+        if (tid < R) rcur[tid] += rcnt[tid];
+    }
+}
+
+// Persistent grid over the slices of MSM_RSORT_SLICE entries of every range's span (a range's last slice may be shorter).  A slice:
+// counting sort by bucket in shared memory (ranks from shared atomics, kept in registers), one global atomic per non-empty bucket
+// to claim that many places in the bucket, and a linear pass that writes each bucket's run contiguously.
+static constexpr int MSM_RSORT_CTAS_PER_SM = 2;     // one CTA's barriers overlap the other's loads
+static __global__ void __launch_bounds__(MSM_SORT_THREADS, MSM_RSORT_CTAS_PER_SM) msm_range_sort_kernel(const uint32_t *__restrict__ offsets, uint32_t nb,
+                                                                              const uint2 *__restrict__ parts, uint32_t *__restrict__ cursor,
+                                                                              uint32_t *__restrict__ sorted) {
+    __shared__ uint32_t sp[MSM_MAX_RANGES + 1];
+    __shared__ uint32_t hist[MSM_RANGE_BUCKETS], start[MSM_RANGE_BUCKETS], base[MSM_RANGE_BUCKETS];
+    __shared__ uint32_t obuf[MSM_RSORT_SLICE];
+    __shared__ uint8_t obkt[MSM_RSORT_SLICE];
+    const uint32_t tid = threadIdx.x, R = msm_ranges(nb);
+    {   // slices per range -> their exclusive prefix sp[0..R]
+        uint32_t s = 0;
+        if (tid < R) s = (offsets[min(nb, (tid + 1) * MSM_RANGE_BUCKETS)] - offsets[tid * MSM_RANGE_BUCKETS] + MSM_RSORT_SLICE - 1) / MSM_RSORT_SLICE;
+        uint32_t total;
+        const uint32_t ex = block_exclusive_scan_1024(s, &total);
+        if (tid < R) sp[tid] = ex;
+        if (tid == 0) sp[R] = total;
+        __syncthreads();
+    }
+    for (uint32_t u = blockIdx.x; u < sp[R]; u += gridDim.x) {
+        uint32_t j0 = 0, j1 = R;                  // the range: largest j with sp[j] <= u
+        while (j1 - j0 > 1) { const uint32_t m = (j0 + j1) >> 1; if (sp[m] <= u) j0 = m; else j1 = m; }
+        const uint32_t r0 = j0 * MSM_RANGE_BUCKETS, rb = min(MSM_RANGE_BUCKETS, nb - r0);
+        const uint32_t lo = offsets[r0] + (u - sp[j0]) * MSM_RSORT_SLICE, hi = min(lo + MSM_RSORT_SLICE, offsets[r0 + rb]);
+        if (tid < MSM_RANGE_BUCKETS) hist[tid] = 0;
+        __syncthreads();
+        uint32_t word[MSM_RSORT_PER_THREAD], key[MSM_RSORT_PER_THREAD];   // key = bucket in range | rank in bucket << 8
+#pragma unroll
+        for (uint32_t e = 0; e < MSM_RSORT_PER_THREAD; e++) {
+            const uint32_t p = lo + e * MSM_SORT_THREADS + tid;
+            key[e] = ~0u;                         // past the slice
+            if (p < hi) {
+                const uint2 v = parts[p];
+                const uint32_t lb = v.y - r0;
+                word[e] = v.x;
+                key[e] = lb | atomicAdd(hist + lb, 1u) << 8;
+            }
+        }
+        __syncthreads();
+        if (tid < 32) {   // exclusive scan of the <= 128 bucket counts, four per lane
+            uint32_t v[MSM_RANGE_BUCKETS / 32], sum = 0;
+#pragma unroll
+            for (uint32_t q = 0; q < MSM_RANGE_BUCKETS / 32; q++) { v[q] = hist[tid * (MSM_RANGE_BUCKETS / 32) + q]; sum += v[q]; }
+            uint32_t incl = sum;
+            for (int d = 1; d < 32; d <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, incl, d); if (tid >= (uint32_t)d) incl += t; }
+            uint32_t run = incl - sum;
+#pragma unroll
+            for (uint32_t q = 0; q < MSM_RANGE_BUCKETS / 32; q++) { start[tid * (MSM_RANGE_BUCKETS / 32) + q] = run; run += v[q]; }
+        }
+        if (tid < rb && hist[tid]) base[tid] = offsets[r0 + tid] + atomicAdd(cursor + r0 + tid, hist[tid]);
+        __syncthreads();
+#pragma unroll
+        for (uint32_t e = 0; e < MSM_RSORT_PER_THREAD; e++) {
+            if (key[e] != ~0u) {
+                const uint32_t lb = key[e] & 0xffu, q = start[lb] + (key[e] >> 8);
+                obuf[q] = word[e];
+                obkt[q] = (uint8_t)lb;
+            }
+        }
+        __syncthreads();
+        for (uint32_t q = tid; q < hi - lo; q += MSM_SORT_THREADS) {
+            const uint32_t lb = obkt[q];
+            sorted[base[lb] + q - start[lb]] = obuf[q];
+        }
+        __syncthreads();                          // hist, start, base and the buffers are reused by the next slice
     }
 }
 
@@ -750,7 +924,7 @@ __global__ void __launch_bounds__(256) msm_bases_to_mont_kernel(Fb *coords, size
 
 // ----------------------------------------------------------------------------- context
 struct MsmScratch {
-    DevBuf counts, hist, offsets, tiles, sorted, buckets, ppt, chunks, chunk_sums, slices, wins, result, scalars, pair_offs[2], pair_pts[2];
+    DevBuf counts, hist, offsets, tiles, sorted, parts, buckets, ppt, chunks, chunk_sums, slices, wins, result, scalars, pair_offs[2], pair_pts[2];
     void *h_wins = nullptr;   // pinned
     void *h_stage[2] = {nullptr, nullptr};          // pinned staging for host-buffer scalars
     cudaEvent_t stage_done[2] = {nullptr, nullptr};
@@ -868,7 +1042,8 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     const uint32_t t1_alloc = std::max(t1, P.t1);
     // a long bucket holds more than MSM_LONG_PARTIALS segment starts, so there are at most t1 / (MSM_LONG_PARTIALS + 1)
     const uint32_t max_long = t1 / (MSM_LONG_PARTIALS + 1) + 1;
-    // digit sort: per-CTA shared-memory histograms when one bucket set fits a CTA's shared memory (see msm_hist_smem_kernel).
+    // digit sort: per-CTA shared-memory histograms and two coalesced passes when one bucket set fits a CTA's shared memory (see
+    // msm_hist_smem_kernel).
     // LURK_MSM_SORT=legacy forces the global-atomics kernels (tuning aid, read at every launch so that one process can compare both)
     const char *sort_env = getenv("LURK_MSM_SORT");
     const bool smem_sort = fixed && (size_t)P.nb * sizeof(uint32_t) <= MSM_SORT_SMEM_MAX && !(sort_env && !strcmp(sort_env, "legacy"));
@@ -877,7 +1052,10 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
         // scratch grows monotonically; a context is normally run at one size (the circuit's witness length)
         auto ensure = [](DevBuf &b, size_t bytes) { return b.bytes >= bytes ? LURK_OK : b.alloc(bytes); };
         LURK_TRY(ensure(S.counts, (((size_t)TB + 1) * 2 + 1 + max_long) * sizeof(uint32_t)));   // counts | cursor | long count | long list
-        if (smem_sort) LURK_TRY(ensure(S.hist, (size_t)sort_ctas * P.nb * sizeof(uint32_t)));   // cnt[G][nb]
+        if (smem_sort) {
+            LURK_TRY(ensure(S.hist, (size_t)sort_ctas * (P.nb + msm_ranges(P.nb)) * sizeof(uint32_t)));   // cnt[G][nb] | rng[G][R]
+            LURK_TRY(ensure(S.parts, n * (size_t)P.nwin * sizeof(uint2)));   // (sorted word, bucket) grouped by bucket range
+        }
         LURK_TRY(ensure(S.offsets, ((size_t)TB + 1) * sizeof(uint32_t)));
         LURK_TRY(ensure(S.tiles, ((size_t)ntiles + 1) * 2 * sizeof(uint32_t)));  // tile sums | tile offsets
         LURK_TRY(ensure(S.sorted, n * (size_t)P.nwin * sizeof(uint32_t)));
@@ -907,28 +1085,33 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     const Fs *sub = (!readback && fmt == LURK_FMT_MONTGOMERY) ? (const Fs *)ctx->d_sub : nullptr;
     if (smem_sort) {
         const size_t smem = (size_t)P.nb * sizeof(uint32_t);
-        uint32_t *cnt = S.hist.as<uint32_t>();
-        if (smem > ((size_t)48 << 10)) {   // above the default limit a kernel opts in, per device
-            LURK_CUDA_TRY(cudaFuncSetAttribute(msm_hist_smem_kernel<Fs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            LURK_CUDA_TRY(cudaFuncSetAttribute(msm_scatter_smem_kernel<Fs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        }
-        LURK_CUDA_TRY(cudaMemsetAsync(long_list - 1, 0, sizeof(uint32_t), s));     // every count is written: only the long-list length is cleared
-        msm_hist_smem_kernel<Fs><<<sort_ctas, MSM_SORT_THREADS, smem, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, P.nb, cnt);
-        msm_hist_columns_kernel<<<(P.nb + 255) / 256, 256, 0, s>>>(cnt, sort_ctas, P.nb, counts);
+        const uint32_t ts = msm_part_scalars(P.nwin);
+        const size_t part_smem = (size_t)ts * P.nwin * (sizeof(uint32_t) + sizeof(uint16_t));
+        uint32_t *cnt = S.hist.as<uint32_t>(), *rng = cnt + (size_t)sort_ctas * P.nb;
+        uint2 *parts = S.parts.as<uint2>();
+        // above the default limit a kernel opts in, per device
+        if (smem > ((size_t)48 << 10)) LURK_CUDA_TRY(cudaFuncSetAttribute(msm_hist_smem_kernel<Fs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if (part_smem > ((size_t)48 << 10))
+            LURK_CUDA_TRY(cudaFuncSetAttribute(msm_partition_kernel<Fs>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)part_smem));
+        // every count is written; only the long-list length is cleared, and the scan's tile sums by the histogram kernel's CTA 0
+        LURK_CUDA_TRY(cudaMemsetAsync(long_list - 1, 0, sizeof(uint32_t), s));
+        msm_hist_smem_kernel<Fs><<<sort_ctas, MSM_SORT_THREADS, smem, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, P.nb, cnt, rng, tile_sums, ntiles);
+        msm_hist_columns_kernel<<<(P.nb + 255) / 256, 256, 0, s>>>(cnt, rng, sort_ctas, P.nb, counts, cursor, tile_sums);
+        msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
+        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, rounds ? nullptr : long_list);
+        msm_partition_kernel<Fs><<<sort_ctas, MSM_SORT_THREADS, part_smem, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, P.nb, ts, base_stride,
+                                                                                 offsets, rng, parts);
+        msm_range_sort_kernel<<<MSM_RSORT_CTAS_PER_SM * sm_count(), MSM_SORT_THREADS, 0, s>>>(offsets, P.nb, parts, cursor, sorted);
         launches++;
     } else {
         LURK_CUDA_TRY(cudaMemsetAsync(counts, 0, (((size_t)TB + 1) * 2 + 1) * sizeof(uint32_t), s));
         msm_count_kernel<Fs><<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, counts);
-    }
-    msm_scan_tile_sums_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_sums);
-    msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
-    // the offsets the accumulation walks also give the merge its long buckets (after the last pair round, if any)
-    msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, rounds ? nullptr : long_list);
-    if (smem_sort)
-        msm_scatter_smem_kernel<Fs><<<sort_ctas, MSM_SORT_THREADS, (size_t)P.nb * sizeof(uint32_t), s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, P.nb, base_stride,
-                                                                                                       offsets, S.hist.as<uint32_t>(), sorted);
-    else
+        msm_scan_tile_sums_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_sums);
+        msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
+        // the offsets the accumulation walks also give the merge its long buckets (after the last pair round, if any)
+        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, rounds ? nullptr : long_list);
         msm_scatter_kernel<Fs><<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, base_stride, offsets, cursor, sorted);
+    }
     if (ctx->profile) LURK_CUDA_TRY(cudaEventRecord(ctx->ev0, s));
     // ---- pair rounds
     const uint32_t *acc_offs = offsets;

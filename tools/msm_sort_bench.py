@@ -5,7 +5,7 @@
   W2 - D    911 900 scalars, 36 % non-zero, window 16 (commit(W2 - D); the vector is generated already reduced by D, so the second
             32-byte load and the subtraction the fold context's sort performs for it are NOT in these numbers)
 
-The time is the span between the CUDA events the commitment context records before the sort's memset and after its scatter kernel
+The time is the span between the CUDA events the commitment context records before the sort's first kernel (or memset) and after its last kernel
 (lurk_msm_ctx_last_sort_ms).  Algorithmic bytes: each of the two passes reads every 32-byte scalar, the scatter writes 4 bytes per
 non-zero digit (counted as windows x non-zero scalars, an upper bound); the bound is those bytes at the H100 SXM data sheet's 3.35 TB/s.
 
