@@ -565,6 +565,18 @@ int lurk_compress_verify(int n_primary, lurk_spartan_ctx *const *primary, lurk_s
  * commitment, HyperKZG's P and Q -- for callers that compose the verifier themselves.  points: count x 96 bytes of the header's form, scalars:
  * count x 32 bytes, out: 96 bytes, all `fmt`.  Host only; works without a GPU. */
 int lurk_point_combination(int curve_id, const uint8_t *points_xyz, const uint8_t *scalars, size_t count, int fmt, uint8_t out_xyz[96]);
+/* n_groups independent combinations on the GPU, in order on `stream`; returns when they are done.
+ * Group g has counts[g] >= 1 terms. Its terms come after the terms of groups 0..g-1 in points_xyz
+ * (total x 96 bytes, host, in the header's form) and scalars (total x 32, fmt).
+ * out_xyz: n_groups x 96 bytes, the same bytes lurk_point_combination writes for that group.
+ * One CTA per group: Straus with 4-bit windows, the tables and window sums spread over its threads, the 252 doublings on one thread.
+ * At most LURK_POINT_COMBINATION_MAX_TERMS terms per group (past it, commit through an lurk_msm_ctx instead).  n_groups < 1, a count
+ * of 0 or over the limit, null pointers, an unknown curve or format are LURK_ERR_ARG; then LURK_ERR_NOGPU without a device; then a
+ * point off the curve or not of the header's form, or a scalar >= r, is LURK_ERR_RANGE with lurk_point_combination's message and the
+ * group's index -- all before anything is launched.  Keeps no state between calls: host threads may call it at once on their streams. */
+#define LURK_POINT_COMBINATION_MAX_TERMS 4096
+int lurk_point_combination_batch(int curve_id, int n_groups, const uint32_t *counts, const uint8_t *points_xyz, const uint8_t *scalars, int fmt,
+                                 uint8_t *out_xyz, void *stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * S5  Fold helpers on device-resident vectors (Arecibo NIFS::prove / R1CSShape::commit_T /

@@ -8,7 +8,7 @@ commitment key); it never computes on the CPU -- every call goes to the CUDA lib
 from . import _capi, compress, recursive, spartan
 from ._capi import (CURVE_BN254_G1, CURVE_GRUMPKIN, CURVE_PALLAS, CURVE_VESTA, FIELD_BN254_FQ, FIELD_BN254_FR,
                     FIELD_PALLAS_FP, FIELD_PALLAS_FQ, FMT_CANONICAL, FMT_MONTGOMERY, LurkError)
-from .compress import CompressContext, compress_prove, compress_verify
+from .compress import CompressContext, compress_prove, compress_verify, point_combination_batch
 from .recursive import recursive_verify
 from .commit import (CommitmentKey, ShardedCommitmentKey, ck_size, from_label, hash_to_curve_batch, point_sum, shake256, shard_bounds,
                      synthetic_bases)

@@ -10,6 +10,7 @@ FIELD_BN254_FR, FIELD_BN254_FQ, FIELD_PALLAS_FQ, FIELD_PALLAS_FP = 0, 1, 2, 3
 CURVE_BN254_G1, CURVE_GRUMPKIN, CURVE_PALLAS, CURVE_VESTA = 0, 1, 2, 3
 FMT_CANONICAL, FMT_MONTGOMERY = 0, 1
 OK, ERR_ARG, ERR_CUDA, ERR_OOM, ERR_RANGE, ERR_NOGPU, ERR_ORDER = 0, -1, -2, -3, -4, -5, -6
+POINT_COMBINATION_MAX_TERMS = 4096
 
 
 class LurkError(RuntimeError):
@@ -178,6 +179,7 @@ PROTOTYPES = {
                                   C.POINTER(_vp), _vp, _vp, _vp, _vp, C.POINTER(CompressProof), _i, COMPRESS_CHALLENGE_FN, PAIRING_CHECK_FN, _vp, _i,
                                   C.POINTER(CompressVerdict), C.POINTER(_i), _i, _vp]),
     "lurk_point_combination": (_i, [_i, _vp, _vp, _sz, _i, _vp]),
+    "lurk_point_combination_batch": (_i, [_i, _i, _vp, _vp, _vp, _i, _vp, _vp]),
     "lurk_recursive_verify_dev": (_i, [_i, C.POINTER(RecursiveInstance), C.POINTER(RecursiveVerdict), C.POINTER(_i), _i, _vp]),
     "lurk_recursive_verify": (_i, [_i, C.POINTER(RecursiveInstance), C.POINTER(RecursiveVerdict), C.POINTER(_i), _i, _vp]),
     "lurk_ipa_verify_dev": (_i, [_i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, CHALLENGE_FN, _vp, C.POINTER(_i), _vp, _vp, _i, _vp]),

@@ -240,3 +240,39 @@ def compress_verify(primary, secondary, pcs_primary, pcs_secondary, instances, i
         raise errors[0]
     _capi.check(rc)
     return bool(acc.value), [(v.snark_ok, v.eval_ok, v.opening_ok) for v in verdicts]
+
+
+def point_combination_batch(curve, groups, fmt=_capi.FMT_CANONICAL, stream=0):
+    """sum_j s_j P_j for each group, all groups in one lurk_point_combination_batch call on the GPU (ordered on `stream`; returns when
+    done).  groups: [(points, scalars)] with 1 .. POINT_COMBINATION_MAX_TERMS terms each -- points as k x 96 bytes x | y | z of the
+    header's form and scalars as k x 32 bytes, both in `fmt` (uint8 arrays), or, in FMT_CANONICAL, as lists of (x, y) / None and of
+    ints.  Returns an (n_groups, 96) uint8 array: per group the bytes lurk_point_combination writes (decode canonical ones with
+    points_of)."""
+    counts, pts, scs = [], [], []
+    for points, scalars in groups:
+        if not isinstance(points, np.ndarray) or not isinstance(scalars, np.ndarray):
+            assert fmt == _capi.FMT_CANONICAL, "lists of points and scalars are canonical integers"
+        p = np.ascontiguousarray(points, dtype=np.uint8).reshape(-1) if isinstance(points, np.ndarray) else list(points)
+        s = np.ascontiguousarray(scalars, dtype=np.uint8).reshape(-1) if isinstance(scalars, np.ndarray) else list(scalars)
+        p = _point_list(p) if isinstance(p, list) and p else p          # an empty list stays empty, and is refused below
+        s = _fes(s) if isinstance(s, list) and s else s
+        k = len(p) // 96
+        if k == 0 or len(p) != 96 * k or len(s) != 32 * k:
+            raise ValueError(f"a group needs k >= 1 points of 96 bytes and k scalars of 32 bytes, got {len(p)} and {len(s)} bytes")
+        counts.append(k)
+        pts.append(p)
+        scs.append(s)
+    if not counts:
+        raise ValueError("at least one group")
+    c = np.array(counts, dtype=np.uint32)
+    p, s = np.concatenate(pts), np.concatenate(scs)
+    out = np.zeros((len(counts), 96), dtype=np.uint8)
+    _capi.check(_capi.lib().lurk_point_combination_batch(curve, len(counts), _capi.np_ptr(c), _capi.np_ptr(p), _capi.np_ptr(s), fmt,
+                                                          _capi.np_ptr(out), C.c_void_p(stream)))
+    return out
+
+
+def points_of(out):
+    """canonical 96-byte points (as point_combination_batch returns them) -> [(x, y) or None]"""
+    b = np.ascontiguousarray(out, dtype=np.uint8).reshape(-1)
+    return _points(b, len(b) // 96)

@@ -1,10 +1,10 @@
 // N4 -- the compress context (include/lurk_b200.h, "Compress context"): CompressedSNARK::prove (reference src/proof/nova.rs:341-356,
 // supernova.rs:293-317) as one C-ABI call.  Per circuit: the Spartan prover of spartan.cu writes the joint polynomial of batch_eval_reduce
-// straight into the opening's arena (P_0 of HyperKZG's fold chain, or a of the inner-product argument), the host forms the joint
-// commitment sum_i weights_i C_i (2n points, ipa.cu's host Straus), and the opening runs on the arena (kzg.cu / ipa.cu).  The primary and
-// the secondary circuit run at once on two library-owned host threads -- Arecibo's rayon::join(S1::prove, S2::prove) -- which keep their
-// thread-local reduction scratch (sc_scratch.cuh) for the life of the context.  No kernels of its own: every device step is one of the
-// existing provers'.
+// straight into the opening's arena (P_0 of HyperKZG's fold chain, or a of the inner-product argument), the joint commitment
+// sum_i weights_i C_i is formed (2n points, point_combination_groups of pointcomb.cu), and the opening runs on the arena (kzg.cu /
+// ipa.cu).  The primary and the secondary circuit run at once on two library-owned host threads -- Arecibo's rayon::join(S1::prove,
+// S2::prove) -- which keep their thread-local reduction scratch (sc_scratch.cuh) for the life of the context.  No kernels of its own:
+// every device step is one of the existing provers'.
 #include "common.cuh"
 #include "pcs.cuh"
 #include "sc_scratch.cuh"
@@ -72,7 +72,8 @@ static int prove_circuit(Circuit &c, int idx, const CircuitInputs &in, lurk_comp
     std::vector<const uint8_t *> pts(2 * (size_t)in.n);
     for (int i = 0; i < in.n; i++) { pts[i] = in.comm_W[i]; pts[in.n + i] = in.comm_E[i]; }
     uint8_t comm[96];
-    LURK_TRY(point_combination(c.curve, pts.data(), weights.data(), 2 * in.n, fmt, comm));
+    const PointGroup joint{pts.data(), weights.data(), 2 * in.n, comm};
+    LURK_TRY(point_combination_groups(c.curve, &joint, 1, fmt, false, s));
     if (out && out->comm) memcpy(out->comm, comm, 96);
     if (c.kind == LURK_PCS_HYPERKZG)
         return hyperkzg_prove_arena(c.curve, c.ck.c, c.arena, d_joint, r.data(), c.m, pcs_challenge, &cc, out ? out->com : nullptr, out ? out->w : nullptr,

@@ -1,8 +1,9 @@
 // N4 -- the compressed verifier (include/lurk_b200.h, "Compressed verifier"): CompressedSNARK::verify (reference src/proof/nova.rs:358-373,
 // supernova.rs:304-317) as one C-ABI call, for the proof lurk_compress_prove_dev writes.  Per circuit: the Spartan verifier of spartan.cu
-// (its one device step is the matrix-evaluation pass), the joint commitment sum_i weights_i C_i (ipa.cu's host Straus), then the opening:
-// the inner-product verifier of ipa.cu on eq(r) in stream-ordered scratch, or HyperKZG's verifier -- the fold consistency of the evaluations
-// and the two G1 points of the batched pairing check, host arithmetic only; the pairing itself is the caller's callback.  The secondary
+// (its one device step is the matrix-evaluation pass), then the opening: the joint commitment sum_i weights_i C_i and the inner-product
+// verifier of ipa.cu on eq(r) in stream-ordered scratch, or HyperKZG's verifier -- the fold consistency of the evaluations and the two G1
+// points of the batched pairing check, the joint commitment folded into the first; the pairing itself is the caller's callback.  The point
+// combinations go through point_combination_groups (pointcomb.cu): the device for the long ones, the host Straus for the short.  The secondary
 // circuit runs on a pooled library thread and a stream forked from the caller's while the primary runs on the calling thread -- Arecibo's
 // rayon::join of S1::verify and S2::verify.  No kernels of its own.
 #include "msm_impl.cuh"
@@ -125,9 +126,11 @@ int check_side_ranges(const Side &c, int rounds_fmt, int fmt) {
 }
 
 // HyperKZG's verifier (provider::hyperkzg::EvaluationEngine::verify) on the host, the pairing left to the callback
+// (the joint commitment comm = sum_i weights_i C_i never reaches HyperKZG's transcript: its term dsum comm of P is taken as the terms
+// dsum weights_i C_i)
 template <class F>
-int hyperkzg_verify(const Side &c, const Transcript &t, const uint8_t comm[96], const uint8_t *r_bytes, const uint8_t je_bytes[32],
-                    lurk_pairing_check_fn pairing, int fmt, lurk_compress_verdict &v) {
+int hyperkzg_verify(const Side &c, const Transcript &t, const uint8_t *weights, const uint8_t *r_bytes, const uint8_t je_bytes[32],
+                    lurk_pairing_check_fn pairing, int fmt, lurk_compress_verdict &v, cudaStream_t s) {
     const lurk_compress_circuit_proof &p = *c.proof;
     const int l = c.m;
     F r, q, d, je;
@@ -148,15 +151,22 @@ int hyperkzg_verify(const Side &c, const Transcript &t, const uint8_t comm[96], 
     if (!v.eval_ok) return LURK_OK;
     LURK_TRY(ask_pcs<F>(t, 1, p.v, 3 * (size_t)l * 32, fmt, q));
     LURK_TRY(ask_pcs<F>(t, 2, p.w, 3 * 96, fmt, d));
-    // P = sum_t d^t (B - B(u_t) G + u_t w_t) over [com_0 = comm, com_1 .., G, w_0, w_1, w_2];  Q = sum_t d^t w_t
+    // P = sum_t d^t (B - B(u_t) G + u_t w_t) over [com_0 = comm = sum_i weights_i C_i, com_1 .., G, w_0, w_1, w_2];  Q = sum_t d^t w_t
     const F u[3] = {r, r.neg(), r.sqr()}, dt[3] = {F::one(), d, d.sqr()};
     const F dsum = dt[0] + dt[1] + dt[2];
-    std::vector<const uint8_t *> pts;
+    std::vector<const uint8_t *> pts(c.comms);
     std::vector<F> sc;
+    for (size_t i = 0; i < c.comms.size(); i++) {
+        F wi;
+        fe_in(weights + 32 * i, fmt, wi);
+        sc.push_back(dsum * wi);
+    }
     F qj = F::one(), bu = F::zero();
     for (int j = 0; j < l; j++, qj = qj * q) {
-        pts.push_back(j ? p.com + 96 * (size_t)(j - 1) : comm);
-        sc.push_back(dsum * qj);
+        if (j) {
+            pts.push_back(p.com + 96 * (size_t)(j - 1));
+            sc.push_back(dsum * qj);
+        }
         for (int k = 0; k < 3; k++) bu += dt[k] * qj * val[(size_t)k * l + j];
     }
     uint8_t g96[96] = {0};
@@ -173,9 +183,9 @@ int hyperkzg_verify(const Side &c, const Transcript &t, const uint8_t comm[96], 
     std::vector<uint8_t> sb(32 * sc.size());
     for (size_t k = 0; k < sc.size(); k++) fe_out(sc[k], fmt, sb.data() + 32 * k);
     uint8_t P[96], Q[96], db[96];
-    LURK_TRY(point_combination(c.curve, pts.data(), sb.data(), (int)pts.size(), fmt, P));
     for (int k = 0; k < 3; k++) fe_out(dt[k], fmt, db + 32 * k);
-    LURK_TRY(point_combination(c.curve, pts.data() + l + 1, db, 3, fmt, Q));
+    const PointGroup pq[2] = {{pts.data(), sb.data(), (int)pts.size(), P}, {pts.data() + pts.size() - 3, db, 3, Q}};
+    LURK_TRY(point_combination_groups(c.curve, pq, 2, fmt, false, s));
     int holds = 0;
     const int rc = pairing(t.user, c.idx, P, Q, &holds);
     if (rc != 0) { set_error("pairing callback failed (%d)", rc); return LURK_ERR_ARG; }
@@ -198,11 +208,12 @@ int verify_side(const Side &c, lurk_compress_challenge_fn fn, lurk_pairing_check
     LURK_TRY(spartan_verify_checked(c.n, c.sp.data(), c.u, c.X.data(), &sp, rounds_fmt, snark_challenge, &t, &acc, fmt, s, c.batched));
     v.snark_ok = acc;
     if (!acc) return LURK_OK;
-    uint8_t comm[96];
-    LURK_TRY(point_combination(c.curve, c.comms.data(), weights.data(), (int)c.comms.size(), fmt, comm));
     if (c.pcs->kind == LURK_PCS_HYPERKZG)
-        return dispatch_field(c.field, [&](auto f) { return hyperkzg_verify<decltype(f)>(c, t, comm, r.data(), je, pairing, fmt, v); });
+        return dispatch_field(c.field, [&](auto f) { return hyperkzg_verify<decltype(f)>(c, t, weights.data(), r.data(), je, pairing, fmt, v, s); });
     // IPA: comm | joint_eval -> the scale of ck_c;  b = eq(r)
+    uint8_t comm[96];
+    const PointGroup joint{c.comms.data(), weights.data(), (int)c.comms.size(), comm};
+    LURK_TRY(point_combination_groups(c.curve, &joint, 1, fmt, false, s));
     uint8_t msg[128], rb[32], gc[64];
     memcpy(msg, comm, 96);
     memcpy(msg + 96, je, 32);

@@ -35,16 +35,6 @@ __global__ void __launch_bounds__(128) ipa_fold_bases_kernel(Affine<F> *g, size_
     }
 }
 
-template <class Fb>
-static void point_to_bytes_fmt(const XYZZ<Fb> &p, int fmt, uint8_t out[96]) {
-    memset(out, 0, 96);
-    if (p.is_identity()) return;
-    Affine<Fb> a = p.to_affine();
-    Fb one = Fb::one();
-    if (fmt == LURK_FMT_CANONICAL) { a.x = a.x.to_canonical(); a.y = a.y.to_canonical(); one = one.to_canonical(); }
-    memcpy(out, a.x.v, 32); memcpy(out + 32, a.y.v, 32); memcpy(out + 64, one.v, 32);
-}
-
 // Fixed-base multiplication of ck_c on the host (the c_L ck_c / c_R ck_c terms, 2 per round): 4-bit windows, 64 mixed additions
 // per product instead of a 254-step double-and-add.
 template <class Fb>
@@ -215,18 +205,6 @@ __global__ void __launch_bounds__(256) ipa_s_kernel(const __grid_constant__ IpaS
     grid_sum<F, 1>(acc, a.partial, a.counter, a.result);
 }
 
-// a 96-byte point x | y | z of the header's convention (z = 1, or x = y = z = 0 for the identity), on the curve y^2 = x^3 + b
-template <class Fb>
-static bool point_in(const uint8_t *in, int fmt, const Fb &b, XYZZ<Fb> &out) {
-    Affine<Fb> p;
-    Fb z;
-    if (!fe_in(in, fmt, p.x) || !fe_in(in + 32, fmt, p.y) || !fe_in(in + 64, fmt, z)) return false;
-    if (z.is_zero()) { out = XYZZ<Fb>::identity(); return p.x.is_zero() && p.y.is_zero(); }
-    if (z != Fb::one() || p.y.sqr() != p.x.sqr() * p.x + b) return false;
-    out = XYZZ<Fb>::from_affine(p);
-    return true;
-}
-
 // sum_{lo <= k < hi} scalars[k] P_k on the host: Straus, 4-bit windows, the 252 doublings shared by all terms of the range
 template <class Fb, class Fs>
 static XYZZ<Fb> host_straus(const std::vector<XYZZ<Fb>> &pts, const std::vector<Fs> &scalars, size_t lo, size_t hi) {
@@ -321,9 +299,10 @@ static int ipa_verify(lurk_msm_ctx *ck, const uint8_t *gc_bytes, const uint8_t *
         sc[2 + 2 * j] = r * r;
         sc[3 + 2 * j] = r_inv * r_inv;
     }
-    // s and b_hat, then ck_hat = commit(ck, s) on the key context.  b_hat is read as soon as the s pass ends, so that the host's side of
-    // the check, Q = comm + (c - a_hat b_hat) ck_c + sum_j (r_j^2 L_j + r_j^-2 R_j), is computed while the commitment runs; after it only
-    // a_hat ck_hat == Q is left.
+    // s and b_hat, then ck_hat = commit(ck, s) on the key context.  b_hat is read as soon as the s pass ends, so that the other side of
+    // the check, Q = comm + (c - a_hat b_hat) ck_c + sum_j (r_j^2 L_j + r_j^-2 R_j), is computed while the commitment runs -- by the
+    // point-combination kernel on a stream of the greatest priority, whose one CTA takes the first SM the commitment's kernels free (or by
+    // the host Straus, for a short Q); after it only a_hat ck_hat == Q is left.
     const size_t n = (size_t)1 << log_n;
     StreamBuf sbuf;
     LURK_TRY(sbuf.alloc(n * sizeof(Fs), s));
@@ -348,9 +327,23 @@ static int ipa_verify(lurk_msm_ctx *ck, const uint8_t *gc_bytes, const uint8_t *
     LURK_CUDA_TRY(cudaEventSynchronize(s_done.e));
     const Fs b_hat = *static_cast<const Fs *>(scr.pinned);
     sc[1] = c - a_hat * b_hat;
-    const XYZZ<Fb> q = host_msm(pts, sc);
+    std::vector<const uint8_t *> q_pts{comm_bytes, gc3};
+    for (int j = 0; j < log_n; j++) {
+        q_pts.push_back(L + 96 * (size_t)j);
+        q_pts.push_back(R + 96 * (size_t)j);
+    }
+    std::vector<uint8_t> q_sc(32 * sc.size());
+    for (size_t k = 0; k < sc.size(); k++) fe_out(sc[k], fmt, q_sc.data() + 32 * k);
+    uint8_t q_bytes[96];
+    const PointGroup q_group{q_pts.data(), q_sc.data(), (int)q_pts.size(), q_bytes};
+    StreamGuard q_stream;
+    int q_rc = q_stream.create_urgent();
+    if (q_rc == LURK_OK) q_rc = point_combination_groups(C::ID, &q_group, 1, fmt, false, q_stream.s);
     uint8_t hat[96];
-    LURK_TRY(lurk_msm_ctx_finish(ck, hat));
+    LURK_TRY(lurk_msm_ctx_finish(ck, hat));            // the key context is left with nothing pending, whatever became of Q
+    LURK_TRY(q_rc);
+    XYZZ<Fb> q;
+    point_in(q_bytes, fmt, b, q);
     XYZZ<Fb> ck_hat = XYZZ<Fb>::identity();
     Fb z;
     memcpy(z.v, hat + 64, 32);
@@ -374,12 +367,6 @@ int ipa_verify_checked(int curve_id, lurk_msm_ctx *ck, const uint8_t *gc_bytes, 
     return dispatch_curve(curve_id, [&](auto cv) {
         return ipa_verify<decltype(cv)>(ck, gc_bytes, comm, c, d_b, log_n, L, R, a_final, challenge, user, accepted, nullptr, nullptr, fmt, s);
     });
-}
-
-template <class C>
-static typename C::Base curve_b() {
-    const Affine<typename C::Base> g = curve_generator<C>();
-    return g.y.sqr() - g.x.sqr() * g.x;
 }
 
 bool points_valid(int curve_id, const uint8_t *const *points, int count, int fmt) {

@@ -43,6 +43,34 @@ int ipa_prove_arena(int curve_id, lurk_msm_ctx *ck, PcsArena &a, const uint8_t *
 int ipa_verify_checked(int curve_id, lurk_msm_ctx *ck, const uint8_t *gc_bytes, const uint8_t *comm, const uint8_t *c, const void *d_b, int log_n,
                        const uint8_t *L, const uint8_t *R, const uint8_t *a_final, lurk_challenge_fn challenge, void *user, int *accepted, int fmt,
                        cudaStream_t s);
+// b of y^2 = x^3 + b
+template <class C>
+static typename C::Base curve_b() {
+    const Affine<typename C::Base> g = curve_generator<C>();
+    return g.y.sqr() - g.x.sqr() * g.x;
+}
+// a 96-byte point x | y | z of the header's convention (z = 1, or x = y = z = 0 for the identity), on the curve y^2 = x^3 + b
+template <class Fb>
+static bool point_in(const uint8_t *in, int fmt, const Fb &b, XYZZ<Fb> &out) {
+    Affine<Fb> p;
+    Fb z;
+    if (!fe_in(in, fmt, p.x) || !fe_in(in + 32, fmt, p.y) || !fe_in(in + 64, fmt, z)) return false;
+    if (z.is_zero()) { out = XYZZ<Fb>::identity(); return p.x.is_zero() && p.y.is_zero(); }
+    if (z != Fb::one() || p.y.sqr() != p.x.sqr() * p.x + b) return false;
+    out = XYZZ<Fb>::from_affine(p);
+    return true;
+}
+// the point in that form: x | y | 1, or 0 | 0 | 0
+template <class Fb>
+static void point_to_bytes_fmt(const XYZZ<Fb> &p, int fmt, uint8_t out[96]) {
+    memset(out, 0, 96);
+    if (p.is_identity()) return;
+    Affine<Fb> a = p.to_affine();
+    Fb one = Fb::one();
+    if (fmt == LURK_FMT_CANONICAL) { a.x = a.x.to_canonical(); a.y = a.y.to_canonical(); one = one.to_canonical(); }
+    memcpy(out, a.x.v, 32); memcpy(out + 32, a.y.v, 32); memcpy(out + 64, one.v, 32);
+}
+
 // every 96-byte point x | y | z of the header's form (z = 1 on the curve, or the identity 0 | 0 | 0), in `fmt`; host only
 bool points_valid(int curve_id, const uint8_t *const *points, int count, int fmt);
 // an affine point x | y (identity = (0, 0)) of the curve, in `fmt`; host only
@@ -51,5 +79,18 @@ bool affine_valid(int curve_id, const uint8_t *xy, int fmt);
 int point_combination(int curve_id, const uint8_t *const *points, const uint8_t *scalars, int count, int fmt, uint8_t out[96]);
 // r ck_c for the affine ck_c (x | y, `fmt`) and the scalar r (`fmt`) as an affine x | y in `fmt`; host only
 int scale_affine(int curve_id, const uint8_t *xy, const uint8_t *r, int fmt, uint8_t out[64]);
+
+// Batched point combination (pointcomb.cu).  One group: out = sum_k scalars[k] points[k], as point_combination takes and writes them.
+struct PointGroup {
+    const uint8_t *const *points;
+    const uint8_t *scalars;
+    int count;
+    uint8_t *out;
+};
+constexpr int PC_MAX_TERMS = LURK_POINT_COMBINATION_MAX_TERMS;     // per group on the device
+// Every group checked first (the messages of point_combination, with the group's index), then: the groups of at least
+// PC_DEVICE_MIN_TERMS terms (every group with `all_device`) combined by one kernel on `s` while the host combines the others.
+// Returns when all are written; the bytes are point_combination's.
+int point_combination_groups(int curve_id, const PointGroup *groups, int n_groups, int fmt, bool all_device, cudaStream_t s);
 
 }  // namespace lurk

@@ -6,7 +6,18 @@
 namespace lurk {
 
 // RAII for the side streams / cloned commitment contexts that let independent Pippenger passes of one prover call overlap
-struct StreamGuard { cudaStream_t s = nullptr; ~StreamGuard() { if (s) cudaStreamDestroy(s); } int create() { LURK_CUDA_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); return LURK_OK; } };
+struct StreamGuard {
+    cudaStream_t s = nullptr;
+    ~StreamGuard() { if (s) cudaStreamDestroy(s); }
+    int create() { LURK_CUDA_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); return LURK_OK; }
+    // the device's greatest priority: its CTAs are placed before those of default-priority streams as SMs free up
+    int create_urgent() {
+        int least = 0, greatest = 0;
+        LURK_CUDA_TRY(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+        LURK_CUDA_TRY(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, greatest));
+        return LURK_OK;
+    }
+};
 struct EventGuard { cudaEvent_t e = nullptr; ~EventGuard() { if (e) cudaEventDestroy(e); } int create() { LURK_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); return LURK_OK; } };
 struct MsmCloneGuard { lurk_msm_ctx *c = nullptr; ~MsmCloneGuard() { if (c) lurk_msm_ctx_destroy(c); } };
 // stream-ordered scratch, freed (in stream order) when the call returns
