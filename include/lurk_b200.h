@@ -101,6 +101,20 @@ int lurk_bitdecomp_witness_batch(int field_id, const uint8_t *values, size_t n, 
 int lurk_bitdecomp_witness_batch_dev(int field_id, const void *d_values, size_t n, void *d_blocks, int fmt,
                                      void *stream);
 
+/* SHA-256 coprocessor (synthesize_sha256, src/coprocessor/sha256.rs:27-64): the witness of one call with n pointers,
+ * in allocation order: per pointer the aux of to_bits_le_strict of its tag, then of its hash; the aux of bellpepper's
+ * sha256 gadget over their bits; pack_bits' element (the digest's low CAPACITY bits, equal to compute_sha256,
+ * sha256.rs:66-90); allocate_constant's ExprTag::Num.  Bits are 0/1 elements in `fmt`.  The block's length depends on
+ * (field, n) only and is what lurk_sha256_witness_block returns (0: unsupported field or n outside 1..MAX_N).
+ * inputs: count * 2n elements in `fmt`, per pointer tag then hash.  The host call rejects elements >= p (LURK_ERR_RANGE). */
+#define LURK_SHA256_MAX_N 32
+size_t lurk_sha256_witness_block(int field_id, int n);
+int lurk_sha256_witness_batch(int field_id, int n, const uint8_t *inputs, size_t count, uint8_t *aux_out, int fmt);
+int lurk_sha256_witness_batch_dev(int field_id, int n, const void *d_inputs, size_t count, void *d_aux, int fmt, void *stream);
+/* In-place form: block k is written at element offset d_offsets[k] (u64, device) of d_W. */
+int lurk_sha256_witness_scatter_dev(int field_id, int n, const void *d_inputs, size_t count, const uint64_t *d_offsets, void *d_W,
+                                    int fmt, void *stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * S2  DAG hydration.  Replaces StoreCore::hydrate_z_cache / hash_ptr_val_unsafe (src/lem/store_core.rs:199-269)
  *     with the preimage layouts of `impl StoreHasher for PoseidonCache` (src/lem/store.rs:29-78).
@@ -631,6 +645,10 @@ void lurk_fold_ctx_destroy(lurk_fold_ctx *ctx);
  * Poseidon slots, 0 = bit-decomposition slots.  offsets[k] = element offset of block k inside W (the reference's layout:
  * every frame's aux = [its slot blocks | LEM body aux], multiframe.rs:635-712).  Returns the batch index (>= 0). */
 int lurk_fold_ctx_add_slot_batch(lurk_fold_ctx *ctx, int arity, size_t count, const uint64_t *offsets);
+/* One batch of `count` SHA-256 coprocessor calls with n pointers each: stage A writes their witness blocks
+ * (lurk_sha256_witness_block elements) into W at element offsets offsets[k].  Its host buffer holds count * 2n inputs
+ * (per pointer tag, then hash).  Returns the batch index (>= 0), an index of the same host buffers as the slot batches. */
+int lurk_fold_ctx_add_sha256_batch(lurk_fold_ctx *ctx, int n, size_t count, const uint64_t *offsets);
 /* The parts of W2 the host produces (LEM body aux, the augmented-circuit part): up to 4 strided spans of W; the host
  * buffer LURK_FOLD_BUF_GLUE holds them densely, span after span, row after row. */
 typedef struct lurk_fold_span { uint64_t first, row_elems, stride, rows; } lurk_fold_span;
@@ -647,7 +665,8 @@ int lurk_fold_ctx_set_spans(lurk_fold_ctx *ctx, int n_spans, const lurk_fold_spa
 #define LURK_FOLD_RO_T_INF 6
 int lurk_fold_ctx_set_ro(lurk_fold_ctx *ctx, int n_absorb, const int *kinds, int challenge_bits);
 /* Pinned host buffers the caller (the CPU witness generator) fills before stage A of buffer b: `which` >= 0 = preimages
- * of that slot batch (count * arity elements; bit decomposition: count values), or one of the names below. */
+ * of that slot batch (count * arity elements; bit decomposition: count values; SHA-256: count * 2n inputs), or one of
+ * the names below. */
 #define LURK_FOLD_BUF_GLUE (-1) /* the spans, densely                       (witness field)            */
 #define LURK_FOLD_BUF_X2 (-2)   /* public IO of the fresh instance, n_x      (witness field)            */
 #define LURK_FOLD_BUF_RO (-3)   /* 24 elements: position i = CONST value of RO slot i (commitment curve's base field) */

@@ -14,6 +14,7 @@ from .commit import (CommitmentKey, ShardedCommitmentKey, ck_size, from_label, h
                      synthetic_bases)
 from .fold import NovaFoldContext, SuperNovaFoldContext
 from .hash import HashConstants, PoseidonCache
+from .sha256 import Sha256Coprocessor, sha256_witness_batch, witness_block
 from .slots import SlotType, compute_witness_size, generate_slots_witnesses, slot_witness_batch_bytes
 from .store import StoreCore
 from .trie import StandardTrie, Trie
@@ -22,7 +23,8 @@ __all__ = [
     "CommitmentKey", "ShardedCommitmentKey", "NovaFoldContext", "SuperNovaFoldContext", "point_sum", "shard_bounds", "synthetic_bases", "ck_size", "from_label",
     "compress", "CompressContext", "compress_prove", "compress_verify", "recursive", "recursive_verify",
     "hash_to_curve_batch", "shake256", "spartan", "HashConstants", "PoseidonCache", "SlotType",
-    "compute_witness_size", "generate_slots_witnesses", "slot_witness_batch_bytes", "StoreCore", "StandardTrie", "Trie", "LurkError",
+    "compute_witness_size", "generate_slots_witnesses", "slot_witness_batch_bytes",
+    "Sha256Coprocessor", "sha256_witness_batch", "witness_block", "StoreCore", "StandardTrie", "Trie", "LurkError",
     "FIELD_BN254_FR", "FIELD_BN254_FQ", "FIELD_PALLAS_FQ", "FIELD_PALLAS_FP", "CURVE_BN254_G1", "CURVE_GRUMPKIN",
     "CURVE_PALLAS", "CURVE_VESTA", "FMT_CANONICAL", "FMT_MONTGOMERY",
 ]

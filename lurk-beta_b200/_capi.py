@@ -122,6 +122,10 @@ PROTOTYPES = {
     "lurk_bitdecomp_witness_block": (_sz, [_i]),
     "lurk_bitdecomp_witness_batch": (_i, [_i, _vp, _sz, _vp, _i]),
     "lurk_bitdecomp_witness_batch_dev": (_i, [_i, _vp, _sz, _vp, _i, _vp]),
+    "lurk_sha256_witness_block": (_sz, [_i, _i]),
+    "lurk_sha256_witness_batch": (_i, [_i, _i, _vp, _sz, _vp, _i]),
+    "lurk_sha256_witness_batch_dev": (_i, [_i, _i, _vp, _sz, _vp, _i, _vp]),
+    "lurk_sha256_witness_scatter_dev": (_i, [_i, _i, _vp, _sz, _vp, _vp, _i, _vp]),
     "lurk_dag_hash": (_i, [_i, _vp, _sz, _vp, _sz, _vp]),
     "lurk_dag_hash_plan": (_i, [_vp, _sz, _sz, C.POINTER(DagPlan)]),
     "lurk_msm_ctx_create": (_i, [_i, _vp, _sz, _i, C.POINTER(_vp)]),
@@ -191,6 +195,7 @@ PROTOTYPES = {
     "lurk_fold_ctx_create": (_i, [C.POINTER(FoldConfig), _vp, _vp, C.POINTER(_vp)]),
     "lurk_fold_ctx_destroy": (None, [_vp]),
     "lurk_fold_ctx_add_slot_batch": (_i, [_vp, _i, _sz, _vp]),
+    "lurk_fold_ctx_add_sha256_batch": (_i, [_vp, _i, _sz, _vp]),
     "lurk_fold_ctx_set_spans": (_i, [_vp, _i, C.POINTER(FoldSpan)]),
     "lurk_fold_ctx_set_ro": (_i, [_vp, _i, C.POINTER(_i), _i]),
     "lurk_fold_ctx_host_buffer": (_i, [_vp, _i, _i, C.POINTER(_vp), C.POINTER(_sz)]),

@@ -407,11 +407,12 @@ struct FoldSpan { uint64_t first, row_elems, stride, rows; };
 
 struct FoldSlotBatch {
     int arity = 0;                 // 0 = bit decomposition
+    int sha_n = 0;                 // > 0: SHA-256 coprocessor calls with sha_n pointers (2 * sha_n inputs each)
     size_t count = 0;
     DevBuf d_offsets;              // u64 element offsets into W
     DevBuf d_pre[FOLD_MAX_DEPTH];  // preimages / values per fresh buffer
     void *h_pre[FOLD_MAX_DEPTH] = {nullptr, nullptr, nullptr, nullptr};   // pinned
-    size_t bytes() const { return count * (size_t)(arity ? arity : 1) * 32; }
+    size_t bytes() const { return count * (size_t)(sha_n ? 2 * sha_n : (arity ? arity : 1)) * 32; }
 };
 
 struct FoldConfigHost {
@@ -432,6 +433,7 @@ struct FoldCtxBase {
     virtual int init(const FoldConfigHost &cfg, const uint64_t *const row_ptr[3], const uint32_t *const col[3], const uint8_t *const val[3], int fmt,
                      lurk_msm_ctx *ck_w, lurk_msm_ctx *ck_t) = 0;
     virtual int add_slot_batch(int arity, size_t count, const uint64_t *offsets) = 0;
+    virtual int add_sha256_batch(int n, size_t count, const uint64_t *offsets) = 0;
     virtual int set_spans(int n, const FoldSpan *spans) = 0;
     virtual int set_ro(int n_absorb, const int *kinds, int challenge_bits) = 0;
     virtual int host_buffer(int b, int which, void **ptr, size_t *bytes) = 0;

@@ -1,5 +1,6 @@
 // Host side of the fold context for one curve (compiled once per curve: -DLURK_C=<curve>); see foldctx_impl.cuh.
 #include "foldctx_impl.cuh"
+#include "sha256.cuh"
 
 #include <cuda.h>      // types of the green-context driver API only; entry points are resolved at run time
 #include <cstring>
@@ -9,7 +10,9 @@ LURK_MSM_EXTERN(LURK_C)
 #define LURK_FOLD_POSEIDON_EXTERN(F)                                                                          \
     extern template int launch_poseidon<F, true>(int, const void *, size_t, void *, int, int, cudaStream_t, const uint64_t *); \
     extern template int poseidon_instance_info<F>(int, const PoseidonParams<F> **, PoseidonLayout *);        \
-    extern template int launch_bitdecomp<F>(const void *, size_t, void *, int, int, cudaStream_t, const uint64_t *);
+    extern template int launch_bitdecomp<F>(const void *, size_t, void *, int, int, cudaStream_t, const uint64_t *); \
+    extern template size_t sha256_block_len<F>(int);                                                          \
+    extern template int launch_sha256_witness<F>(const void *, size_t, int, void *, const uint64_t *, int, int, cudaStream_t);
 LURK_FOLD_POSEIDON_EXTERN(Fe<Bn254Fr>)
 LURK_FOLD_POSEIDON_EXTERN(Fe<Bn254Fq>)
 LURK_FOLD_POSEIDON_EXTERN(Fe<PallasFq>)
@@ -361,6 +364,18 @@ struct FoldCtx final : FoldCtxBase {
             if (offsets[k] + blk > cfg.n_w) { set_error("slot block %zu does not fit into W", k); return LURK_ERR_ARG; }
         auto sb = std::make_unique<FoldSlotBatch>();
         sb->arity = arity;
+        return add_batch(std::move(sb), count, offsets);
+    }
+    int add_sha256_batch(int n, size_t count, const uint64_t *offsets) override {
+        const size_t blk = sha256_block_len<Fs>(n);
+        if (!blk) { set_error("SHA-256 coprocessor arity %d: 1..%d", n, LURK_SHA256_MAX_N); return LURK_ERR_ARG; }
+        for (size_t k = 0; k < count; k++)
+            if (offsets[k] + blk > cfg.n_w) { set_error("SHA-256 block %zu does not fit into W", k); return LURK_ERR_ARG; }
+        auto sb = std::make_unique<FoldSlotBatch>();
+        sb->sha_n = n;
+        return add_batch(std::move(sb), count, offsets);
+    }
+    int add_batch(std::unique_ptr<FoldSlotBatch> sb, size_t count, const uint64_t *offsets) {
         sb->count = count;
         LURK_TRY(sb->d_offsets.alloc(std::max<size_t>(1, count) * sizeof(uint64_t)));
         if (count) LURK_CUDA_TRY(cudaMemcpy(sb->d_offsets.p, offsets, count * sizeof(uint64_t), cudaMemcpyHostToDevice));
@@ -538,12 +553,12 @@ struct FoldCtx final : FoldCtxBase {
         dummy_ready = true;
         static const bool off = getenv("LURK_FOLD_NO_DUMMY_OFFSET") != nullptr;      // measurement aid
         size_t nslots = 0;
-        for (auto &sb : batches) nslots += sb->count;
+        for (auto &sb : batches) nslots += sb->sha_n ? 0 : sb->count;   // SHA-256 blocks are not part of D
         if (off || !nslots || !cfg.n_w) return LURK_OK;
         LURK_TRY(dummy_w.alloc((size_t)cfg.n_w * sizeof(Fs)));
         LURK_CUDA_TRY(cudaMemsetAsync(dummy_w.p, 0, (size_t)cfg.n_w * sizeof(Fs), sB));
         for (auto &sb : batches) {
-            if (!sb->count) continue;
+            if (!sb->count || sb->sha_n) continue;
             void *zeros = nullptr;
             LURK_CUDA_TRY(cudaMallocAsync(&zeros, sb->bytes(), sB));
             LURK_CUDA_TRY(cudaMemsetAsync(zeros, 0, sb->bytes(), sB));
@@ -613,7 +628,9 @@ struct FoldCtx final : FoldCtxBase {
             cudaStream_t st = sK[idx % 3];
             idx++;
             if (!sb->count) continue;
-            if (sb->arity) {
+            if (sb->sha_n) {
+                LURK_TRY(launch_sha256_witness<Fs>(sb->d_pre[b].p, sb->count, sb->sha_n, W2, sb->d_offsets.as<uint64_t>(), fmt, LURK_FMT_MONTGOMERY, st));
+            } else if (sb->arity) {
                 LURK_TRY((launch_poseidon<Fs, true>(sb->arity, sb->d_pre[b].p, sb->count, W2, fmt, LURK_FMT_MONTGOMERY, st, sb->d_offsets.as<uint64_t>())));
             } else {
                 uint32_t mod[8];

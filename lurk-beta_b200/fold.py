@@ -67,6 +67,16 @@ class NovaFoldContext:
         self.batches.append((arity, offs.size))
         return idx
 
+    def add_sha256_batch(self, n, offsets):
+        """`len(offsets)` SHA-256 coprocessor calls with n pointers each (sha256.py); their witness blocks are written into W
+        at these element offsets.  The batch's host buffer holds their inputs (per pointer tag, then hash); returns its index"""
+        offs = np.ascontiguousarray(offsets, dtype=np.uint64)
+        idx = self.lib.lurk_fold_ctx_add_sha256_batch(self._ctx, n, offs.size, offs.ctypes.data_as(C.c_void_p))
+        if idx < 0:
+            _capi.check(idx)
+        self.batches.append((("sha256", n), offs.size))
+        return idx
+
     def set_spans(self, spans):
         arr = (FoldSpan * len(spans))(*[FoldSpan(*map(int, s)) for s in spans])
         _capi.check(self.lib.lurk_fold_ctx_set_spans(self._ctx, len(spans), arr))
@@ -199,6 +209,10 @@ class SuperNovaFoldContext:
         self.contexts = list(contexts)               # NovaFoldContext per circuit index
         self._next = [0] * len(self.contexts)        # next fresh-instance buffer per circuit
         self._started = [False] * len(self.contexts)
+
+    def add_sha256_batch(self, circuit_index, n, offsets):
+        """SHA-256 coprocessor calls of the circuit `circuit_index` (see NovaFoldContext.add_sha256_batch)"""
+        return self.contexts[circuit_index].add_sha256_batch(n, offsets)
 
     def stage_a(self, circuit_index, **kw):
         c = self.contexts[circuit_index]

@@ -15,6 +15,10 @@ All integers little-endian; field elements 32 bytes canonical (`PrimeField::to_r
                            u32 len | len x 32 bytes }
   commit file: "LRKC" | u32 version=1 | u32 curve (0 BN254 G1, 1 Grumpkin, 2 Pallas, 3 Vesta) | u32 flags | u32 n |
                n x 64 bytes affine bases (x | y; identity = 0 | 0) | n x 32 bytes scalars | 64 bytes affine result | u8 is_identity
+  sha256 file: "LRKH" | u32 version=1 | u32 field | u32 flags | u32 n | 2n x 32 bytes inputs (tag, hash per pointer) |
+               u32 len | len x 32 bytes aux -- one call of the SHA-256 coprocessor's `synthesize_sha256`
+               (src/coprocessor/sha256.rs:27-64) and the aux block it allocated: pins the aux order of
+               lurk_sha256_witness_batch (tests/test_trace_sha256.py).
   key file   : "LRKK" | u32 version=1 | u32 curve | u32 flags | u32 kind (0 = from_label / Pedersen, 1 = powers of tau / KZG) |
                u32 label_len | label | u32 n | n x 64 bytes affine points -- the head of the reference's commitment key as
                `CommitmentKey::setup(label, ..)` produced it (SURVEY.md 8(f) N3): pins lurk_ck_generate (kind 0).  For kind 1 the label
@@ -34,6 +38,7 @@ TRACE_FIELD_TO_ID = {0: 0, 1: 1, 2: 2, 3: 3}
 Slot = namedtuple("Slot", "slot_type is_dummy witness")          # witness: uint8 array, len * 32 bytes
 SlotTrace = namedtuple("SlotTrace", "field_id synthetic slots")
 CommitTrace = namedtuple("CommitTrace", "curve_id synthetic bases scalars result is_identity")
+Sha256Trace = namedtuple("Sha256Trace", "field_id synthetic n inputs aux")   # inputs: 2n * 32 bytes, aux: len * 32 bytes
 KeyTrace = namedtuple("KeyTrace", "curve_id synthetic kind label points")     # points: uint8 array, n * 64 bytes
 
 
@@ -94,6 +99,33 @@ def read_commit(path):
     if off + 65 != len(data):
         raise ValueError(f"{path}: trailing bytes")
     return CommitTrace(curve, bool(flags & FLAG_SYNTHETIC), bases, scalars, result, ident)
+
+
+def write_sha256(path, field_id, n, inputs, aux, synthetic=True):
+    inputs = np.ascontiguousarray(inputs, dtype=np.uint8).reshape(-1)
+    aux = np.ascontiguousarray(aux, dtype=np.uint8).reshape(-1)
+    assert inputs.size == 64 * n and aux.size % 32 == 0
+    with open(path, "wb") as f:
+        f.write(b"LRKH" + struct.pack("<IIII", 1, field_id, FLAG_SYNTHETIC if synthetic else 0, n) + inputs.tobytes())
+        f.write(struct.pack("<I", aux.size // 32) + aux.tobytes())
+
+
+def read_sha256(path):
+    data = open(path, "rb").read()
+    if data[:4] != b"LRKH":
+        raise ValueError(f"{path}: not a SHA-256 trace")
+    version, field, flags, n = struct.unpack_from("<IIII", data, 4)
+    if version != 1 or n < 1:
+        raise ValueError(f"{path}: unknown version / empty call")
+    off = 20
+    inputs = np.frombuffer(data, dtype=np.uint8, count=64 * n, offset=off).copy()
+    off += 64 * n
+    (ln,) = struct.unpack_from("<I", data, off)
+    off += 4
+    aux = np.frombuffer(data, dtype=np.uint8, count=32 * ln, offset=off).copy()
+    if off + 32 * ln != len(data):
+        raise ValueError(f"{path}: trailing bytes")
+    return Sha256Trace(TRACE_FIELD_TO_ID[field], bool(flags & FLAG_SYNTHETIC), n, inputs, aux)
 
 
 def write_key(path, curve_id, kind, label, points, synthetic=True):
