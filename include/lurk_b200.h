@@ -115,6 +115,31 @@ int lurk_sha256_witness_batch_dev(int field_id, int n, const void *d_inputs, siz
 int lurk_sha256_witness_scatter_dev(int field_id, int n, const void *d_inputs, size_t count, const uint64_t *d_offsets, void *d_W,
                                     int fmt, void *stream);
 
+/* Trie coprocessor (src/coprocessor/trie/mod.rs): the witness of one lookup (synthesize_lookup_aux, mod.rs:118-156) or
+ * insert (synthesize_insert_aux, mod.rs:226-268) over an arity-8 trie of height H = 1..LURK_TRIE_MAX_HEIGHT (StandardTrie:
+ * 85), in allocation order, with D = lurk_bitdecomp_witness_block(field_id):
+ *   allocated_root_value | the D - 1 aux of key.to_bits_le_strict | per level L = 0..H-1 (root level first): the 8
+ *   preimage elements, their arity-8 Poseidon aux and digest (the slot block), select's 7 picks (most significant bit
+ *   first: 4, 2, 1; the last pick of level H-1 is the lookup's result)
+ * and, for an insert, then per level L = H-1 down to 0: the new preimage's slot block (the last element is the new root).
+ * Lookup: D + 403 H elements, insert: D + 799 H; lurk_trie_witness_block returns it (0: unsupported field, op or height).
+ * inputs, per call in `fmt`, paths root level first: lookup root, key, path[H][8] (2 + 8H elements); insert root, key,
+ * value, old_path[H][8], new_path[H][8] (3 + 16H) -- the reference's LookupProof / InsertProof preimages.
+ * The host call rejects elements >= p (LURK_ERR_RANGE) and, after the copy back, paths that do not chain
+ * (LURK_ERR_ARG, naming the call and level): each level's digest must equal the element its parent selects (level 0:
+ * root), and for an insert the new path's elements at the key must equal the digest of the level below, the leaf's the
+ * value.  The _dev and scatter forms do not check paths: the caller vouches for them. */
+#define LURK_TRIE_LOOKUP 0
+#define LURK_TRIE_INSERT 1
+#define LURK_TRIE_MAX_HEIGHT 85
+size_t lurk_trie_witness_block(int field_id, int op, int height);
+int lurk_trie_witness_batch(int field_id, int op, int height, const uint8_t *inputs, size_t count, uint8_t *aux_out, int fmt);
+int lurk_trie_witness_batch_dev(int field_id, int op, int height, const void *d_inputs, size_t count, void *d_aux, int fmt,
+                                void *stream);
+/* In-place form: block k is written at element offset d_offsets[k] (u64, device) of d_W. */
+int lurk_trie_witness_scatter_dev(int field_id, int op, int height, const void *d_inputs, size_t count, const uint64_t *d_offsets,
+                                  void *d_W, int fmt, void *stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * S2  DAG hydration.  Replaces StoreCore::hydrate_z_cache / hash_ptr_val_unsafe (src/lem/store_core.rs:199-269)
  *     with the preimage layouts of `impl StoreHasher for PoseidonCache` (src/lem/store.rs:29-78).
@@ -649,6 +674,11 @@ int lurk_fold_ctx_add_slot_batch(lurk_fold_ctx *ctx, int arity, size_t count, co
  * (lurk_sha256_witness_block elements) into W at element offsets offsets[k].  Its host buffer holds count * 2n inputs
  * (per pointer tag, then hash).  Returns the batch index (>= 0), an index of the same host buffers as the slot batches. */
 int lurk_fold_ctx_add_sha256_batch(lurk_fold_ctx *ctx, int n, size_t count, const uint64_t *offsets);
+/* One batch of `count` trie coprocessor calls (op LURK_TRIE_LOOKUP / LURK_TRIE_INSERT, height H): stage A writes their
+ * witness blocks (lurk_trie_witness_block elements) into W at element offsets offsets[k].  Its host buffer holds the
+ * calls' inputs (lurk_trie_witness_batch's layout).  Stage A trusts them as it trusts slot preimages: paths are not
+ * checked.  Returns the batch index (>= 0), an index of the same host buffers as the slot batches. */
+int lurk_fold_ctx_add_trie_batch(lurk_fold_ctx *ctx, int op, int height, size_t count, const uint64_t *offsets);
 /* The parts of W2 the host produces (LEM body aux, the augmented-circuit part): up to 4 strided spans of W; the host
  * buffer LURK_FOLD_BUF_GLUE holds them densely, span after span, row after row. */
 typedef struct lurk_fold_span { uint64_t first, row_elems, stride, rows; } lurk_fold_span;
@@ -665,8 +695,8 @@ int lurk_fold_ctx_set_spans(lurk_fold_ctx *ctx, int n_spans, const lurk_fold_spa
 #define LURK_FOLD_RO_T_INF 6
 int lurk_fold_ctx_set_ro(lurk_fold_ctx *ctx, int n_absorb, const int *kinds, int challenge_bits);
 /* Pinned host buffers the caller (the CPU witness generator) fills before stage A of buffer b: `which` >= 0 = preimages
- * of that slot batch (count * arity elements; bit decomposition: count values; SHA-256: count * 2n inputs), or one of
- * the names below. */
+ * of that slot batch (count * arity elements; bit decomposition: count values; SHA-256: count * 2n inputs; trie: count
+ * calls' inputs), or one of the names below. */
 #define LURK_FOLD_BUF_GLUE (-1) /* the spans, densely                       (witness field)            */
 #define LURK_FOLD_BUF_X2 (-2)   /* public IO of the fresh instance, n_x      (witness field)            */
 #define LURK_FOLD_BUF_RO (-3)   /* 24 elements: position i = CONST value of RO slot i (commitment curve's base field) */

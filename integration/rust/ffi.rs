@@ -16,6 +16,9 @@ pub const LURK_CURVE_PALLAS: c_int = 2;
 pub const LURK_CURVE_VESTA: c_int = 3;
 pub const LURK_FMT_CANONICAL: c_int = 0;
 pub const LURK_FMT_MONTGOMERY: c_int = 1;
+pub const LURK_TRIE_LOOKUP: c_int = 0;
+pub const LURK_TRIE_INSERT: c_int = 1;
+pub const LURK_TRIE_MAX_HEIGHT: c_int = 85;
 pub const LURK_FOLD_BUF_GLUE: c_int = -1;
 pub const LURK_FOLD_BUF_X2: c_int = -2;
 pub const LURK_FOLD_BUF_RO: c_int = -3;
@@ -110,6 +113,13 @@ extern "C" {
     pub fn lurk_poseidon_witness_batch(field_id: c_int, arity: c_int, preimages: *const u8, n: usize, blocks: *mut u8, fmt: c_int) -> c_int;
     pub fn lurk_bitdecomp_witness_block(field_id: c_int) -> usize;
     pub fn lurk_bitdecomp_witness_batch(field_id: c_int, values: *const u8, n: usize, blocks: *mut u8, fmt: c_int) -> c_int;
+    // a12 -- synthesize_lookup_aux / synthesize_insert_aux (src/coprocessor/trie/mod.rs:118-156, 226-268)
+    pub fn lurk_trie_witness_block(field_id: c_int, op: c_int, height: c_int) -> usize;
+    pub fn lurk_trie_witness_batch(field_id: c_int, op: c_int, height: c_int, inputs: *const u8, count: usize, aux_out: *mut u8, fmt: c_int) -> c_int;
+    pub fn lurk_trie_witness_batch_dev(field_id: c_int, op: c_int, height: c_int, d_inputs: *const c_void, count: usize, d_aux: *mut c_void, fmt: c_int,
+                                       stream: *mut c_void) -> c_int;
+    pub fn lurk_trie_witness_scatter_dev(field_id: c_int, op: c_int, height: c_int, d_inputs: *const c_void, count: usize, d_offsets: *const u64,
+                                         d_w: *mut c_void, fmt: c_int, stream: *mut c_void) -> c_int;
     // S2 -- StoreCore::hydrate_z_cache (src/lem/store_core.rs:256-269)
     pub fn lurk_dag_hash(field_id: c_int, nodes: *const lurk_dag_node, n: usize, atom_digests: *const u8, n_atoms: usize, out: *mut u8) -> c_int;
     // S4 -- Arecibo CommitmentEngineTrait::commit (call sites src/proof/nova.rs:287,292)
@@ -121,6 +131,7 @@ extern "C" {
     pub fn lurk_fold_ctx_create(cfg: *const lurk_fold_config, ck_w: *mut lurk_msm_ctx, ck_t: *mut lurk_msm_ctx, out: *mut *mut lurk_fold_ctx) -> c_int;
     pub fn lurk_fold_ctx_destroy(ctx: *mut lurk_fold_ctx);
     pub fn lurk_fold_ctx_add_slot_batch(ctx: *mut lurk_fold_ctx, arity: c_int, count: usize, offsets: *const u64) -> c_int;
+    pub fn lurk_fold_ctx_add_trie_batch(ctx: *mut lurk_fold_ctx, op: c_int, height: c_int, count: usize, offsets: *const u64) -> c_int;
     pub fn lurk_fold_ctx_set_spans(ctx: *mut lurk_fold_ctx, n: c_int, spans: *const lurk_fold_span) -> c_int;
     pub fn lurk_fold_ctx_set_ro(ctx: *mut lurk_fold_ctx, n_absorb: c_int, kinds: *const c_int, challenge_bits: c_int) -> c_int;
     pub fn lurk_fold_ctx_host_buffer(ctx: *mut lurk_fold_ctx, b: c_int, which: c_int, ptr: *mut *mut c_void, bytes: *mut usize) -> c_int;

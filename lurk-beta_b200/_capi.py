@@ -9,6 +9,7 @@ LIB_PATH = os.path.join(_HERE, "liblurk_b200.so")
 FIELD_BN254_FR, FIELD_BN254_FQ, FIELD_PALLAS_FQ, FIELD_PALLAS_FP = 0, 1, 2, 3
 CURVE_BN254_G1, CURVE_GRUMPKIN, CURVE_PALLAS, CURVE_VESTA = 0, 1, 2, 3
 FMT_CANONICAL, FMT_MONTGOMERY = 0, 1
+TRIE_LOOKUP, TRIE_INSERT, TRIE_MAX_HEIGHT = 0, 1, 85
 OK, ERR_ARG, ERR_CUDA, ERR_OOM, ERR_RANGE, ERR_NOGPU, ERR_ORDER = 0, -1, -2, -3, -4, -5, -6
 POINT_COMBINATION_MAX_TERMS = 4096
 
@@ -126,6 +127,10 @@ PROTOTYPES = {
     "lurk_sha256_witness_batch": (_i, [_i, _i, _vp, _sz, _vp, _i]),
     "lurk_sha256_witness_batch_dev": (_i, [_i, _i, _vp, _sz, _vp, _i, _vp]),
     "lurk_sha256_witness_scatter_dev": (_i, [_i, _i, _vp, _sz, _vp, _vp, _i, _vp]),
+    "lurk_trie_witness_block": (_sz, [_i, _i, _i]),
+    "lurk_trie_witness_batch": (_i, [_i, _i, _i, _vp, _sz, _vp, _i]),
+    "lurk_trie_witness_batch_dev": (_i, [_i, _i, _i, _vp, _sz, _vp, _i, _vp]),
+    "lurk_trie_witness_scatter_dev": (_i, [_i, _i, _i, _vp, _sz, _vp, _vp, _i, _vp]),
     "lurk_dag_hash": (_i, [_i, _vp, _sz, _vp, _sz, _vp]),
     "lurk_dag_hash_plan": (_i, [_vp, _sz, _sz, C.POINTER(DagPlan)]),
     "lurk_msm_ctx_create": (_i, [_i, _vp, _sz, _i, C.POINTER(_vp)]),
@@ -196,6 +201,7 @@ PROTOTYPES = {
     "lurk_fold_ctx_destroy": (None, [_vp]),
     "lurk_fold_ctx_add_slot_batch": (_i, [_vp, _i, _sz, _vp]),
     "lurk_fold_ctx_add_sha256_batch": (_i, [_vp, _i, _sz, _vp]),
+    "lurk_fold_ctx_add_trie_batch": (_i, [_vp, _i, _i, _sz, _vp]),
     "lurk_fold_ctx_set_spans": (_i, [_vp, _i, C.POINTER(FoldSpan)]),
     "lurk_fold_ctx_set_ro": (_i, [_vp, _i, C.POINTER(_i), _i]),
     "lurk_fold_ctx_host_buffer": (_i, [_vp, _i, _i, C.POINTER(_vp), C.POINTER(_sz)]),

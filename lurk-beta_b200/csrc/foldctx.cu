@@ -65,6 +65,11 @@ int lurk_fold_ctx_add_sha256_batch(lurk_fold_ctx *ctx, int n, size_t count, cons
     if (count && !offsets) { set_error("null offsets"); return LURK_ERR_ARG; }
     return ctx->impl->add_sha256_batch(n, count, offsets);
 }
+int lurk_fold_ctx_add_trie_batch(lurk_fold_ctx *ctx, int op, int height, size_t count, const uint64_t *offsets) {
+    FOLD_CHECK(ctx);
+    if (count && !offsets) { set_error("null offsets"); return LURK_ERR_ARG; }
+    return ctx->impl->add_trie_batch(op, height, count, offsets);
+}
 int lurk_fold_ctx_set_spans(lurk_fold_ctx *ctx, int n_spans, const lurk_fold_span *spans) {
     FOLD_CHECK(ctx);
     if (n_spans && !spans) { set_error("null spans"); return LURK_ERR_ARG; }

@@ -16,6 +16,7 @@
 #pragma once
 #include "msm_impl.cuh"
 #include "poseidon_api.h"
+#include "trie.cuh"
 #include "spmv3.cuh"
 
 #include <memory>
@@ -408,11 +409,13 @@ struct FoldSpan { uint64_t first, row_elems, stride, rows; };
 struct FoldSlotBatch {
     int arity = 0;                 // 0 = bit decomposition
     int sha_n = 0;                 // > 0: SHA-256 coprocessor calls with sha_n pointers (2 * sha_n inputs each)
+    int trie_op = 0, trie_h = 0;   // trie_h > 0: trie coprocessor calls (trie_n_inputs(trie_op, trie_h) inputs each)
     size_t count = 0;
     DevBuf d_offsets;              // u64 element offsets into W
     DevBuf d_pre[FOLD_MAX_DEPTH];  // preimages / values per fresh buffer
     void *h_pre[FOLD_MAX_DEPTH] = {nullptr, nullptr, nullptr, nullptr};   // pinned
-    size_t bytes() const { return count * (size_t)(sha_n ? 2 * sha_n : (arity ? arity : 1)) * 32; }
+    bool coprocessor() const { return sha_n || trie_h; }   // its blocks are not part of the dummy witness D
+    size_t bytes() const { return count * (sha_n ? 2 * (size_t)sha_n : trie_h ? trie_n_inputs(trie_op, trie_h) : (size_t)(arity ? arity : 1)) * 32; }
 };
 
 struct FoldConfigHost {
@@ -434,6 +437,7 @@ struct FoldCtxBase {
                      lurk_msm_ctx *ck_w, lurk_msm_ctx *ck_t) = 0;
     virtual int add_slot_batch(int arity, size_t count, const uint64_t *offsets) = 0;
     virtual int add_sha256_batch(int n, size_t count, const uint64_t *offsets) = 0;
+    virtual int add_trie_batch(int op, int height, size_t count, const uint64_t *offsets) = 0;
     virtual int set_spans(int n, const FoldSpan *spans) = 0;
     virtual int set_ro(int n_absorb, const int *kinds, int challenge_bits) = 0;
     virtual int host_buffer(int b, int which, void **ptr, size_t *bytes) = 0;

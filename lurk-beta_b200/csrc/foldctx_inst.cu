@@ -8,11 +8,13 @@
 namespace lurk {
 LURK_MSM_EXTERN(LURK_C)
 #define LURK_FOLD_POSEIDON_EXTERN(F)                                                                          \
-    extern template int launch_poseidon<F, true>(int, const void *, size_t, void *, int, int, cudaStream_t, const uint64_t *); \
+    extern template int launch_poseidon<F, true>(int, const void *, size_t, void *, int, int, cudaStream_t, const uint64_t *, const PoseidonGather *); \
     extern template int poseidon_instance_info<F>(int, const PoseidonParams<F> **, PoseidonLayout *);        \
     extern template int launch_bitdecomp<F>(const void *, size_t, void *, int, int, cudaStream_t, const uint64_t *); \
     extern template size_t sha256_block_len<F>(int);                                                          \
-    extern template int launch_sha256_witness<F>(const void *, size_t, int, void *, const uint64_t *, int, int, cudaStream_t);
+    extern template int launch_sha256_witness<F>(const void *, size_t, int, void *, const uint64_t *, int, int, cudaStream_t); \
+    extern template size_t trie_block_len<F>(int, int);                                                       \
+    extern template int launch_trie_witness<F>(int, int, const void *, size_t, void *, const uint64_t *, int, int, cudaStream_t);
 LURK_FOLD_POSEIDON_EXTERN(Fe<Bn254Fr>)
 LURK_FOLD_POSEIDON_EXTERN(Fe<Bn254Fq>)
 LURK_FOLD_POSEIDON_EXTERN(Fe<PallasFq>)
@@ -375,6 +377,16 @@ struct FoldCtx final : FoldCtxBase {
         sb->sha_n = n;
         return add_batch(std::move(sb), count, offsets);
     }
+    int add_trie_batch(int op, int height, size_t count, const uint64_t *offsets) override {
+        const size_t blk = trie_block_len<Fs>(op, height);
+        if (!blk) { set_error("trie op %d / height %d: op 0 (lookup) or 1 (insert), height 1..%d", op, height, LURK_TRIE_MAX_HEIGHT); return LURK_ERR_ARG; }
+        for (size_t k = 0; k < count; k++)
+            if (offsets[k] + blk > cfg.n_w) { set_error("trie block %zu does not fit into W", k); return LURK_ERR_ARG; }
+        auto sb = std::make_unique<FoldSlotBatch>();
+        sb->trie_op = op;
+        sb->trie_h = height;
+        return add_batch(std::move(sb), count, offsets);
+    }
     int add_batch(std::unique_ptr<FoldSlotBatch> sb, size_t count, const uint64_t *offsets) {
         sb->count = count;
         LURK_TRY(sb->d_offsets.alloc(std::max<size_t>(1, count) * sizeof(uint64_t)));
@@ -553,12 +565,12 @@ struct FoldCtx final : FoldCtxBase {
         dummy_ready = true;
         static const bool off = getenv("LURK_FOLD_NO_DUMMY_OFFSET") != nullptr;      // measurement aid
         size_t nslots = 0;
-        for (auto &sb : batches) nslots += sb->sha_n ? 0 : sb->count;   // SHA-256 blocks are not part of D
+        for (auto &sb : batches) nslots += sb->coprocessor() ? 0 : sb->count;   // coprocessor blocks are not part of D
         if (off || !nslots || !cfg.n_w) return LURK_OK;
         LURK_TRY(dummy_w.alloc((size_t)cfg.n_w * sizeof(Fs)));
         LURK_CUDA_TRY(cudaMemsetAsync(dummy_w.p, 0, (size_t)cfg.n_w * sizeof(Fs), sB));
         for (auto &sb : batches) {
-            if (!sb->count || sb->sha_n) continue;
+            if (!sb->count || sb->coprocessor()) continue;
             void *zeros = nullptr;
             LURK_CUDA_TRY(cudaMallocAsync(&zeros, sb->bytes(), sB));
             LURK_CUDA_TRY(cudaMemsetAsync(zeros, 0, sb->bytes(), sB));
@@ -630,6 +642,10 @@ struct FoldCtx final : FoldCtxBase {
             if (!sb->count) continue;
             if (sb->sha_n) {
                 LURK_TRY(launch_sha256_witness<Fs>(sb->d_pre[b].p, sb->count, sb->sha_n, W2, sb->d_offsets.as<uint64_t>(), fmt, LURK_FMT_MONTGOMERY, st));
+            } else if (sb->trie_h) {
+                LURK_TRY(launch_trie_witness<Fs>(sb->trie_op, sb->trie_h, sb->d_pre[b].p, sb->count, W2, sb->d_offsets.as<uint64_t>(), fmt,
+                                                 LURK_FMT_MONTGOMERY, st));
+                k++;   // two launches: the Poseidon levels, then root, bits and picks
             } else if (sb->arity) {
                 LURK_TRY((launch_poseidon<Fs, true>(sb->arity, sb->d_pre[b].p, sb->count, W2, fmt, LURK_FMT_MONTGOMERY, st, sb->d_offsets.as<uint64_t>())));
             } else {

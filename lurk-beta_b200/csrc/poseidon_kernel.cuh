@@ -117,10 +117,24 @@ __device__ __forceinline__ void matvec(const SpongeState<F> &S, const F *M, int 
     }
 }
 
+// element offsets of sponge h's preimage and witness block (see PoseidonGather)
+template <int ARITY>
+__device__ __forceinline__ void gather_at(const PoseidonGather &G, size_t h, const uint64_t *__restrict__ offs, size_t &pre, size_t &blk) {
+    if (G.per_call == 1) {
+        pre = h * G.in_stride + G.in_first;
+        blk = (offs ? offs[h] : h * G.out_stride) + G.out0;
+        return;
+    }
+    const size_t c = h / (unsigned)G.per_call;
+    const int l = (int)(h - c * (unsigned)G.per_call);
+    pre = c * G.in_stride + G.in_first + (size_t)ARITY * l;
+    blk = (offs ? offs[c] : c * G.out_stride) + (l < G.split ? G.out0 + G.step0 * l : G.out1 + G.step1 * (l - G.split));
+}
+
 template <class F, int ARITY, bool WITNESS>
 __global__ void __launch_bounds__(ARITY >= 6 ? 384 : 512)
 poseidon_kernel(const F *__restrict__ g_consts, PoseidonLayout L, F tag, const F *__restrict__ pre, size_t n,
-                F *__restrict__ out, const uint64_t *__restrict__ offs, int in_fmt, int out_fmt) {
+                F *__restrict__ out, const uint64_t *__restrict__ offs, PoseidonGather G, int in_fmt, int out_fmt) {
     constexpr int T = ARITY + 1;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t mbar;
@@ -142,8 +156,10 @@ poseidon_kernel(const F *__restrict__ g_consts, PoseidonLayout L, F tag, const F
 
     const int half = L.rf / 2;
     for (size_t h = (size_t)blockIdx.x * blockDim.x + tid; h < n; h += (size_t)gridDim.x * blockDim.x) {
-        const F *p = pre + h * ARITY;
-        F *wout = WITNESS ? out + (offs ? offs[h] : h * (size_t)L.block_elems) : nullptr;
+        size_t pre_at, blk_at;
+        gather_at<ARITY>(G, h, offs, pre_at, blk_at);
+        const F *p = pre + pre_at;
+        F *wout = WITNESS ? out + blk_at : nullptr;
         AuxSink<F, WITNESS> aux;
         aux.next = wout + ARITY;
         aux.fmt = out_fmt;
@@ -233,7 +249,7 @@ __device__ __forceinline__ F shfl_down_fe(const F &x, int d) {
 template <class F, int ARITY, bool WITNESS>
 __global__ void __launch_bounds__(128)
 poseidon_warp_kernel(const F *__restrict__ g_consts, PoseidonLayout L, F tag, const F *__restrict__ pre, size_t n,
-                     F *__restrict__ out, const uint64_t *__restrict__ offs, int in_fmt, int out_fmt) {
+                     F *__restrict__ out, const uint64_t *__restrict__ offs, PoseidonGather G, int in_fmt, int out_fmt) {
     constexpr int T = ARITY + 1;
     constexpr int GPW = 32 / T;   // sponges per warp
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -257,12 +273,14 @@ poseidon_warp_kernel(const F *__restrict__ g_consts, PoseidonLayout L, F tag, co
     const bool live = g < GPW && h < n;                // idle lanes run the same code on zeros and never store
     const int half = L.rf / 2;
 
-    F *wout = (WITNESS && live) ? out + (offs ? offs[h] : h * (size_t)L.block_elems) : nullptr;
+    size_t pre_at = 0, blk_at = 0;
+    if (live) gather_at<ARITY>(G, h, offs, pre_at, blk_at);
+    F *wout = (WITNESS && live) ? out + blk_at : nullptr;
     const bool mont_out = out_fmt == LURK_FMT_MONTGOMERY;
     // absorb
     F s = tag;
     if (i > 0) {
-        F raw = live ? load_fe<F>(pre + h * ARITY + (i - 1)) : F::zero();
+        F raw = live ? load_fe<F>(pre + pre_at + (i - 1)) : F::zero();
         s = in_fmt == LURK_FMT_MONTGOMERY ? raw : F::from_canonical(raw);
         if (WITNESS && live) store_fe(wout + (i - 1), mont_out ? s : (in_fmt == LURK_FMT_MONTGOMERY ? s.to_canonical() : raw));
     }
@@ -338,24 +356,18 @@ poseidon_warp_kernel(const F *__restrict__ g_consts, PoseidonLayout L, F tag, co
 // aux order of bellpepper-core AllocatedNum::to_bits_le_strict (call site src/lem/circuit.rs:241-243) preceded by
 // the slot's preimage element: walking the bits of p-1 from the top, a bit under a 1 of p-1 is allocated and
 // joins the current run; at the first 0 after a run the run (plus the previous run result) is AND-folded, one
-// aux per AND, then the bit is allocated.  Output values are 0/1 field elements.
+// aux per AND, then the bit is allocated.  Output values are 0/1 field elements.  bitdecomp_aux writes the aux of
+// canonical x, the block without its leading value: o[0 .. block - 1).
 template <class F>
-__global__ void bitdecomp_kernel(const F *__restrict__ vals, size_t n, F *__restrict__ out, const uint64_t *__restrict__ offs,
-                                 int block_elems, int in_fmt, int out_fmt) {
+__device__ void bitdecomp_aux(const F &x, F *o, int out_fmt) {
     using P = typename F::Params;
-    size_t h = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (h >= n) return;
-    F raw = load_fe<F>(vals + h);
-    F x = in_fmt == LURK_FMT_MONTGOMERY ? raw.to_canonical() : raw;
-    F *o = out + (offs ? offs[h] : h * (size_t)block_elems);
     const F one = out_fmt == LURK_FMT_MONTGOMERY ? F::one() : F::from_u64(1).to_canonical();
     const F zero = F::zero();
-    store_fe(o, out_fmt == LURK_FMT_MONTGOMERY ? (in_fmt == LURK_FMT_MONTGOMERY ? raw : F::from_canonical(raw)) : x);
     uint32_t b[8];
     b[0] = P::MOD(0) - 1;   // p is odd: no borrow
 #pragma unroll
     for (int i = 1; i < 8; i++) b[i] = P::MOD(i);
-    int k = 1;
+    int k = 0;
     bool found = false, have_last = false;
     uint32_t last = 0;
     int run_len = 0;
@@ -384,6 +396,18 @@ __global__ void bitdecomp_kernel(const F *__restrict__ vals, size_t n, F *__rest
             store_fe(o + k++, ab ? one : zero);   // AllocatedBit::alloc_conditionally
         }
     }
+}
+
+template <class F>
+__global__ void bitdecomp_kernel(const F *__restrict__ vals, size_t n, F *__restrict__ out, const uint64_t *__restrict__ offs,
+                                 int block_elems, int in_fmt, int out_fmt) {
+    size_t h = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= n) return;
+    F raw = load_fe<F>(vals + h);
+    F x = in_fmt == LURK_FMT_MONTGOMERY ? raw.to_canonical() : raw;
+    F *o = out + (offs ? offs[h] : h * (size_t)block_elems);
+    store_fe(o, out_fmt == LURK_FMT_MONTGOMERY ? (in_fmt == LURK_FMT_MONTGOMERY ? raw : F::from_canonical(raw)) : x);
+    bitdecomp_aux(x, o + 1, out_fmt);
 }
 
 // ----------------------------------------------------------------------------- constant cache + launch
@@ -451,29 +475,31 @@ struct SmemOptIn {
 
 template <class F, int ARITY, bool WITNESS>
 int launch_one(const F *d_consts, const PoseidonInstance<F> &inst, const void *d_pre, size_t n, void *d_out,
-                      const uint64_t *d_offs, int in_fmt, int out_fmt, int grid, int block, cudaStream_t s) {
+                      const uint64_t *d_offs, const PoseidonGather &G, int in_fmt, int out_fmt, int grid, int block, cudaStream_t s) {
     constexpr int T = ARITY + 1;
     constexpr int BIG = ARITY >= 6 ? 384 : 512;
     auto kern = poseidon_kernel<F, ARITY, WITNESS>;
     static SmemOptIn optin;           // per device: opt in to the large dynamic shared-memory carve-out
     LURK_TRY(optin.ensure(kern, (size_t)inst.layout.flat_len * sizeof(F) + (size_t)T * 2 * BIG * sizeof(uint4)));
     size_t smem = (size_t)inst.layout.flat_len * sizeof(F) + (size_t)T * 2 * block * sizeof(uint4);
-    kern<<<grid, block, smem, s>>>(d_consts, inst.layout, inst.params.domain_tag, (const F *)d_pre, n, (F *)d_out, d_offs, in_fmt, out_fmt);
+    kern<<<grid, block, smem, s>>>(d_consts, inst.layout, inst.params.domain_tag, (const F *)d_pre, n, (F *)d_out, d_offs, G, in_fmt, out_fmt);
     LURK_CUDA_TRY(cudaGetLastError());
     return LURK_OK;
 }
 
 template <class F, int ARITY, bool WITNESS>
-int launch_arity(const void *d_pre, size_t n, void *d_out, const uint64_t *d_offs, int in_fmt, int out_fmt, cudaStream_t s) {
+int launch_arity(const void *d_pre, size_t n, void *d_out, const uint64_t *d_offs, const PoseidonGather *g, int in_fmt, int out_fmt,
+                 cudaStream_t s) {
     if (n == 0) return LURK_OK;
     PoseidonInstance<F> &inst = instance<F>(ARITY);
+    const PoseidonGather G = g ? *g : PoseidonGather{1, 1, ARITY, 0, (uint64_t)inst.layout.block_elems, 0, 0, 0, 0};
     const F *d_consts = nullptr;
     LURK_TRY(device_consts(inst, &d_consts));
     const int sms = sm_count();
     constexpr int BIG = ARITY >= 6 ? 384 : 512;
     if (n >= (size_t)sms * BIG / 2) {
         // throughput shape: one persistent CTA per SM
-        return launch_one<F, ARITY, WITNESS>(d_consts, inst, d_pre, n, d_out, d_offs, in_fmt, out_fmt, sms, BIG, s);
+        return launch_one<F, ARITY, WITNESS>(d_consts, inst, d_pre, n, d_out, d_offs, G, in_fmt, out_fmt, sms, BIG, s);
     }
     if (n <= 8192) {
         // latency shape (the slot batches of one fold, one level of the store DAG): warp-per-sponge kernel
@@ -484,7 +510,7 @@ int launch_arity(const void *d_pre, size_t n, void *d_out, const uint64_t *d_off
         const size_t smem = (size_t)inst.layout.flat_len * sizeof(F);
         static SmemOptIn optin;
         LURK_TRY(optin.ensure(kern, smem));
-        kern<<<grid, 128, smem, s>>>(d_consts, inst.layout, inst.params.domain_tag, (const F *)d_pre, n, (F *)d_out, d_offs, in_fmt, out_fmt);
+        kern<<<grid, 128, smem, s>>>(d_consts, inst.layout, inst.params.domain_tag, (const F *)d_pre, n, (F *)d_out, d_offs, G, in_fmt, out_fmt);
         LURK_CUDA_TRY(cudaGetLastError());
         return LURK_OK;
     }
@@ -492,16 +518,17 @@ int launch_arity(const void *d_pre, size_t n, void *d_out, const uint64_t *d_off
     // constants once, so one-warp CTAs are used only when there are fewer warps than SMs x 2)
     const int block = n >= (size_t)sms * 128 ? 128 : (n >= (size_t)sms * 64 ? 64 : 32);
     int grid = (int)((n + block - 1) / block);
-    return launch_one<F, ARITY, WITNESS>(d_consts, inst, d_pre, n, d_out, d_offs, in_fmt, out_fmt, grid, block, s);
+    return launch_one<F, ARITY, WITNESS>(d_consts, inst, d_pre, n, d_out, d_offs, G, in_fmt, out_fmt, grid, block, s);
 }
 
 template <class F, bool WITNESS>
-int launch_poseidon(int arity, const void *d_pre, size_t n, void *d_out, int in_fmt, int out_fmt, cudaStream_t s, const uint64_t *d_offs) {
+int launch_poseidon(int arity, const void *d_pre, size_t n, void *d_out, int in_fmt, int out_fmt, cudaStream_t s, const uint64_t *d_offs,
+                    const PoseidonGather *g) {
     switch (arity) {
-        case 3: return launch_arity<F, 3, WITNESS>(d_pre, n, d_out, d_offs, in_fmt, out_fmt, s);
-        case 4: return launch_arity<F, 4, WITNESS>(d_pre, n, d_out, d_offs, in_fmt, out_fmt, s);
-        case 6: return launch_arity<F, 6, WITNESS>(d_pre, n, d_out, d_offs, in_fmt, out_fmt, s);
-        case 8: return launch_arity<F, 8, WITNESS>(d_pre, n, d_out, d_offs, in_fmt, out_fmt, s);
+        case 3: return launch_arity<F, 3, WITNESS>(d_pre, n, d_out, d_offs, g, in_fmt, out_fmt, s);
+        case 4: return launch_arity<F, 4, WITNESS>(d_pre, n, d_out, d_offs, g, in_fmt, out_fmt, s);
+        case 6: return launch_arity<F, 6, WITNESS>(d_pre, n, d_out, d_offs, g, in_fmt, out_fmt, s);
+        case 8: return launch_arity<F, 8, WITNESS>(d_pre, n, d_out, d_offs, g, in_fmt, out_fmt, s);
     }
     set_error("unsupported Poseidon arity %d (HashArity is 3, 4, 6 or 8; src/hash.rs:11-29)", arity);
     return LURK_ERR_ARG;

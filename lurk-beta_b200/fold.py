@@ -77,6 +77,17 @@ class NovaFoldContext:
         self.batches.append((("sha256", n), offs.size))
         return idx
 
+    def add_trie_batch(self, op, height, offsets):
+        """`len(offsets)` trie coprocessor calls (op trie.TRIE_LOOKUP / TRIE_INSERT at this height); their witness blocks
+        are written into W at these element offsets.  The batch's host buffer holds their inputs (trie.lookup_inputs /
+        insert_inputs), which stage A trusts: paths are not checked.  Returns its index"""
+        offs = np.ascontiguousarray(offsets, dtype=np.uint64)
+        idx = self.lib.lurk_fold_ctx_add_trie_batch(self._ctx, op, height, offs.size, offs.ctypes.data_as(C.c_void_p))
+        if idx < 0:
+            _capi.check(idx)
+        self.batches.append((("trie", op, height), offs.size))
+        return idx
+
     def set_spans(self, spans):
         arr = (FoldSpan * len(spans))(*[FoldSpan(*map(int, s)) for s in spans])
         _capi.check(self.lib.lurk_fold_ctx_set_spans(self._ctx, len(spans), arr))
@@ -213,6 +224,10 @@ class SuperNovaFoldContext:
     def add_sha256_batch(self, circuit_index, n, offsets):
         """SHA-256 coprocessor calls of the circuit `circuit_index` (see NovaFoldContext.add_sha256_batch)"""
         return self.contexts[circuit_index].add_sha256_batch(n, offsets)
+
+    def add_trie_batch(self, circuit_index, op, height, offsets):
+        """trie coprocessor calls of the circuit `circuit_index` (see NovaFoldContext.add_trie_batch)"""
+        return self.contexts[circuit_index].add_trie_batch(op, height, offsets)
 
     def stage_a(self, circuit_index, **kw):
         c = self.contexts[circuit_index]

@@ -19,6 +19,10 @@ All integers little-endian; field elements 32 bytes canonical (`PrimeField::to_r
                u32 len | len x 32 bytes aux -- one call of the SHA-256 coprocessor's `synthesize_sha256`
                (src/coprocessor/sha256.rs:27-64) and the aux block it allocated: pins the aux order of
                lurk_sha256_witness_batch (tests/test_trace_sha256.py).
+  trie file  : "LRKT" | u32 version=1 | u32 field | u32 flags | u32 op (0 lookup, 1 insert) | u32 height | u32 n_in |
+               n_in x 32 bytes inputs | u32 len | len x 32 bytes aux -- one call of the trie coprocessor's
+               synthesize_lookup_aux / synthesize_insert_aux (src/coprocessor/trie/mod.rs:118-156, 226-268), its inputs as
+               lurk_trie_witness_batch takes them and the aux block it allocated (tests/test_trace_trie.py).
   key file   : "LRKK" | u32 version=1 | u32 curve | u32 flags | u32 kind (0 = from_label / Pedersen, 1 = powers of tau / KZG) |
                u32 label_len | label | u32 n | n x 64 bytes affine points -- the head of the reference's commitment key as
                `CommitmentKey::setup(label, ..)` produced it (SURVEY.md 8(f) N3): pins lurk_ck_generate (kind 0).  For kind 1 the label
@@ -39,6 +43,7 @@ Slot = namedtuple("Slot", "slot_type is_dummy witness")          # witness: uint
 SlotTrace = namedtuple("SlotTrace", "field_id synthetic slots")
 CommitTrace = namedtuple("CommitTrace", "curve_id synthetic bases scalars result is_identity")
 Sha256Trace = namedtuple("Sha256Trace", "field_id synthetic n inputs aux")   # inputs: 2n * 32 bytes, aux: len * 32 bytes
+TrieTrace = namedtuple("TrieTrace", "field_id synthetic op height inputs aux")   # inputs: n_in * 32 bytes, aux: len * 32
 KeyTrace = namedtuple("KeyTrace", "curve_id synthetic kind label points")     # points: uint8 array, n * 64 bytes
 
 
@@ -126,6 +131,33 @@ def read_sha256(path):
     if off + 32 * ln != len(data):
         raise ValueError(f"{path}: trailing bytes")
     return Sha256Trace(TRACE_FIELD_TO_ID[field], bool(flags & FLAG_SYNTHETIC), n, inputs, aux)
+
+
+def write_trie(path, field_id, op, height, inputs, aux, synthetic=True):
+    inputs = np.ascontiguousarray(inputs, dtype=np.uint8).reshape(-1)
+    aux = np.ascontiguousarray(aux, dtype=np.uint8).reshape(-1)
+    assert inputs.size % 32 == 0 and aux.size % 32 == 0
+    with open(path, "wb") as f:
+        f.write(b"LRKT" + struct.pack("<IIIIII", 1, field_id, FLAG_SYNTHETIC if synthetic else 0, op, height, inputs.size // 32))
+        f.write(inputs.tobytes() + struct.pack("<I", aux.size // 32) + aux.tobytes())
+
+
+def read_trie(path):
+    data = open(path, "rb").read()
+    if data[:4] != b"LRKT":
+        raise ValueError(f"{path}: not a trie trace")
+    version, field, flags, op, height, n_in = struct.unpack_from("<IIIIII", data, 4)
+    if version != 1 or op not in (0, 1) or height < 1:
+        raise ValueError(f"{path}: unknown version / op / height")
+    off = 28
+    inputs = np.frombuffer(data, dtype=np.uint8, count=32 * n_in, offset=off).copy()
+    off += 32 * n_in
+    (ln,) = struct.unpack_from("<I", data, off)
+    off += 4
+    aux = np.frombuffer(data, dtype=np.uint8, count=32 * ln, offset=off).copy()
+    if off + 32 * ln != len(data):
+        raise ValueError(f"{path}: trailing bytes")
+    return TrieTrace(TRACE_FIELD_TO_ID[field], bool(flags & FLAG_SYNTHETIC), op, height, inputs, aux)
 
 
 def write_key(path, curve_id, kind, label, points, synthetic=True):

@@ -6,10 +6,24 @@ method names as the reference: `path` (mod.rs:589-609), `empty_root` (485-497), 
 `insert` (745-776), `prove_lookup_at_path` (725-743).  The evaluation side hashes through
 `PoseidonCache::compute_hash` (hash.rs:97-113) and records preimages in an inverse cache, exactly like the reference;
 `lookup_circuit_witnesses` produces the 85 arity-8 slot witnesses the lookup circuit allocates (SURVEY.md 8(a) a12) in
-ONE batched launch -- the 85 hashes of a path are independent once the preimages are known."""
+ONE batched launch -- the 85 hashes of a path are independent once the preimages are known.
+
+The lookup and insert circuits' whole aux blocks (synthesize_lookup_aux, mod.rs:118-156; synthesize_insert_aux,
+226-268) are written on the GPU from the calls' proofs (`prove_lookup` / `prove_insert`, mod.rs:718-776):
+`lookup_inputs` / `insert_inputs` pack a call, `trie_witness_batch` writes the blocks (include/lurk_b200.h,
+lurk_trie_witness_*), and the fold context writes them straight into W (NovaFoldContext.add_trie_batch)."""
+from collections import namedtuple
+
+import numpy as np
+
+from . import _capi
 from .hash import PoseidonCache
 from .slots import SlotType, slot_witness_batch_bytes
 from .field import pack
+
+TRIE_LOOKUP, TRIE_INSERT = _capi.TRIE_LOOKUP, _capi.TRIE_INSERT
+LookupProof = namedtuple("LookupProof", "preimage_path")            # root level first, ARITY elements each
+InsertProof = namedtuple("InsertProof", "old_proof new_proof")      # LookupProofs before and after the insert
 
 
 class Trie:
@@ -60,6 +74,26 @@ class Trie:
             nxt = pre[k]
         return preimages
 
+    def prove_lookup(self, key):
+        """the preimages on the key's path, root level first; the last one holds the payload (mod.rs:718-743)"""
+        return LookupProof(self.prove_lookup_at_path(self.path(key)))
+
+    def prove_insert(self, key, value):
+        """insert and return (InsertProof(old, new), inserted): the path's preimages before and after (mod.rs:751-811)"""
+        path = self.path(key)
+        old = self.prove_lookup_at_path(path)
+        value = int(value)
+        new = []
+        for k, existing in zip(reversed(path), reversed(old)):
+            new_pre = list(existing)
+            new_pre[k] = value
+            value = self.register_hash(new_pre)
+            new.append(tuple(new_pre))
+        new.reverse()
+        inserted = value != self.root
+        self.root = value
+        return InsertProof(LookupProof(old), LookupProof(new)), inserted
+
     def lookup_aux(self, key):
         path = self.path(key)
         return self.prove_lookup_at_path(path)[-1][path[-1]]
@@ -69,16 +103,7 @@ class Trie:
         return None if v == self.empty_element() else v
 
     def insert(self, key, value):
-        path = self.path(key)
-        old = self.prove_lookup_at_path(path)
-        value = int(value)
-        for k, existing in zip(reversed(path), reversed(old)):
-            new_pre = list(existing)
-            new_pre[k] = value
-            value = self.register_hash(new_pre)
-        inserted = value != self.root
-        self.root = value
-        return inserted
+        return self.prove_insert(key, value)[1]
 
     def lookup_circuit_witnesses(self, key, fmt=0):
         """the HEIGHT arity-8 Poseidon witnesses of synthesize_lookup (mod.rs:654-724) as one batch: uint8 array of
@@ -90,3 +115,40 @@ class Trie:
 
 def StandardTrie(poseidon_cache=None, root=None, inverse_cache=None):
     return Trie(poseidon_cache, 8, 85, root, inverse_cache)
+
+
+def lookup_inputs(root, key, proof):
+    """one lookup call's inputs: root, key, the proof's preimages root level first (2 + 8H elements, ints)"""
+    return [int(root), int(key)] + [int(x) for pre in proof.preimage_path for x in pre]
+
+
+def insert_inputs(root, key, value, proof):
+    """one insert call's inputs: the root before the insert, key, value, the old path, the new path (3 + 16H elements)"""
+    return ([int(root), int(key), int(value)] + [int(x) for pre in proof.old_proof.preimage_path for x in pre]
+            + [int(x) for pre in proof.new_proof.preimage_path for x in pre])
+
+
+def trie_n_inputs(op, height):
+    return 3 + 16 * height if op == TRIE_INSERT else 2 + 8 * height
+
+
+def trie_witness_block(field_id, op, height):
+    """elements of the witness block of one lookup (op TRIE_LOOKUP) or insert (TRIE_INSERT) call at this height"""
+    size = _capi.lib().lurk_trie_witness_block(field_id, op, height)
+    if not size:
+        raise ValueError(f"no trie witness for field {field_id}, op {op} and height {height}")
+    return size
+
+
+def trie_witness_batch(field_id, op, height, inputs, fmt=_capi.FMT_CANONICAL):
+    """inputs: uint8 array of count calls' inputs (lookup_inputs / insert_inputs, packed) -> uint8 array of count
+    witness blocks.  Raises LurkError (ERR_ARG, naming the call and level) when a call's paths do not chain."""
+    blk = trie_witness_block(field_id, op, height)
+    src = np.ascontiguousarray(inputs, dtype=np.uint8).reshape(-1)
+    per = 32 * trie_n_inputs(op, height)
+    if src.size % per:
+        raise ValueError("input buffer is not a whole number of calls")
+    count = src.size // per
+    out = np.zeros(count * blk * 32, dtype=np.uint8)
+    _capi.check(_capi.lib().lurk_trie_witness_batch(field_id, op, height, _capi.np_ptr(src), count, _capi.np_ptr(out), fmt))
+    return out
