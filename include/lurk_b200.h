@@ -17,8 +17,13 @@
  *   - Ownership: the caller owns every buffer.  Contexts are created/destroyed by paired calls.
  *   - Errors: 0 = LURK_OK, negative = error; lurk_last_error() returns a thread-local message.  The library
  *     never aborts or unwinds (reference error style: Result<_, ProofError>, src/error.rs:8-18).
- *   - Threading: every call is re-entrant; `*_dev` calls are asynchronous on the given CUDA stream
- *     (a cudaStream_t passed as void*; NULL = default stream), host-buffer calls synchronise before returning.
+ *   - Threading: every call is re-entrant.  A `*_dev` call reads its device inputs in the order of the given CUDA stream (a
+ *     cudaStream_t passed as void*; NULL = the legacy default stream): work queued on that stream before the call is complete before the
+ *     call reads, also on the side streams some calls fork from it.  "Asynchronous" below: the call returns once its work is queued on the
+ *     stream, and its device outputs are ready in the order of that stream.  "Returns when done": the call returns after its device work,
+ *     its side streams' included, has finished, so its outputs may be read from any stream.  Every `*_dev` entry point says which.  The
+ *     first call of a shape may also wait while it sets up tables or scratch (NTT twiddles, constant tables, MSM scratch growth).
+ *     Host-buffer calls synchronise before returning.
  *   - Non-canonical inputs (>= p) are rejected with LURK_ERR_RANGE by the host-buffer calls (mirrors
  *     from_repr failing, src/field.rs:76-81); `*_dev` calls assume reduced inputs.
  *   - There is no CPU fallback: without a CUDA device every compute call returns LURK_ERR_NOGPU.
@@ -69,6 +74,7 @@ int lurk_field_modulus(int field_id, uint8_t out[32]);
  * ------------------------------------------------------------------------------------------------- */
 int lurk_poseidon_hash_batch(int field_id, int arity, const uint8_t *preimages, size_t n, uint8_t *digests);
 int lurk_poseidon_hash_batch_mont(int field_id, int arity, const uint8_t *preimages, size_t n, uint8_t *digests);
+/* Asynchronous. */
 int lurk_poseidon_hash_batch_dev(int field_id, int arity, const void *d_preimages, size_t n, void *d_digests,
                                  int fmt, void *stream);
 /* Constants as PoseidonConstants::new() builds them (src/hash.rs:61-72): R_F, R_P, the t*(R_F+R_P) round
@@ -87,6 +93,7 @@ int lurk_poseidon_constants(int field_id, int arity, int *full_rounds, int *part
 size_t lurk_poseidon_witness_block(int field_id, int arity);
 int lurk_poseidon_witness_batch(int field_id, int arity, const uint8_t *preimages, size_t n, uint8_t *blocks,
                                 int fmt);
+/* The _dev and _scatter_dev witness forms below are asynchronous. */
 int lurk_poseidon_witness_batch_dev(int field_id, int arity, const void *d_preimages, size_t n, void *d_blocks,
                                     int fmt, void *stream);
 /* In-place form for the step witness: block k is written at element offset d_offsets[k] (u64, device) of d_base.  In the
@@ -106,7 +113,8 @@ int lurk_bitdecomp_witness_batch_dev(int field_id, const void *d_values, size_t 
  * sha256 gadget over their bits; pack_bits' element (the digest's low CAPACITY bits, equal to compute_sha256,
  * sha256.rs:66-90); allocate_constant's ExprTag::Num.  Bits are 0/1 elements in `fmt`.  The block's length depends on
  * (field, n) only and is what lurk_sha256_witness_block returns (0: unsupported field or n outside 1..MAX_N).
- * inputs: count * 2n elements in `fmt`, per pointer tag then hash.  The host call rejects elements >= p (LURK_ERR_RANGE). */
+ * inputs: count * 2n elements in `fmt`, per pointer tag then hash.  The host call rejects elements >= p (LURK_ERR_RANGE).
+ * The _dev and scatter forms are asynchronous. */
 #define LURK_SHA256_MAX_N 32
 size_t lurk_sha256_witness_block(int field_id, int n);
 int lurk_sha256_witness_batch(int field_id, int n, const uint8_t *inputs, size_t count, uint8_t *aux_out, int fmt);
@@ -128,7 +136,7 @@ int lurk_sha256_witness_scatter_dev(int field_id, int n, const void *d_inputs, s
  * The host call rejects elements >= p (LURK_ERR_RANGE) and, after the copy back, paths that do not chain
  * (LURK_ERR_ARG, naming the call and level): each level's digest must equal the element its parent selects (level 0:
  * root), and for an insert the new path's elements at the key must equal the digest of the level below, the leaf's the
- * value.  The _dev and scatter forms do not check paths: the caller vouches for them. */
+ * value.  The _dev and scatter forms do not check paths: the caller vouches for them.  They are asynchronous. */
 #define LURK_TRIE_LOOKUP 0
 #define LURK_TRIE_INSERT 1
 #define LURK_TRIE_MAX_HEIGHT 85
@@ -189,6 +197,7 @@ void lurk_msm_ctx_destroy(lurk_msm_ctx *ctx);
 int lurk_msm_ctx_info(lurk_msm_ctx *ctx, int *curve_id, size_t *n);
 /* sum_{i<n} scalars[i] * bases[i], n <= size of the key */
 int lurk_msm_ctx_run(lurk_msm_ctx *ctx, const uint8_t *scalars, size_t n, int fmt, uint8_t out_xyz[96]);
+/* _dev: returns when done (the point is a host output). */
 int lurk_msm_ctx_run_dev(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, uint8_t out_xyz[96],
                          void *stream);
 /* Fixed-base acceleration (the key never changes between folds): builds table[w][i] = 2^(c w) * bases[i] once
@@ -240,19 +249,21 @@ int lurk_ck_generate(int curve_id, const uint8_t *label, size_t label_len, size_
 /* same, written to device memory in Montgomery form -- exactly what lurk_msm_ctx_create_dev borrows: the key never crosses
  * PCIe.  Returns when the key is complete (the host thread feeds the XOF stream while the GPU works). */
 int lurk_ck_generate_dev(int curve_id, const uint8_t *label, size_t label_len, size_t n, void *d_bases_mont, void *stream);
-/* points first .. first + n - 1 of the same key: a rank's contiguous slice of a key sharded over GPUs (SURVEY.md 8(e)) */
+/* points first .. first + n - 1 of the same key: a rank's contiguous slice of a key sharded over GPUs (SURVEY.md 8(e)); returns when
+ * complete, as lurk_ck_generate_dev */
 int lurk_ck_generate_range_dev(int curve_id, const uint8_t *label, size_t label_len, size_t first, size_t n, void *d_bases_mont,
                                void *stream);
 /* Curve::hash_to_curve(domain_prefix)(message) for n messages of msg_len bytes each (msg_len <= 64 and
  * msg_len + strlen(domain_prefix) <= ~80: everything must fit the single-block layout, else LURK_ERR_ARG). */
 int lurk_hash_to_curve_batch(int curve_id, const char *domain_prefix, const uint8_t *messages, size_t msg_len, size_t n, int fmt,
                              uint8_t *points_out);
+/* _dev: asynchronous. */
 int lurk_hash_to_curve_batch_dev(int curve_id, const char *domain_prefix, const void *d_messages, size_t msg_len, size_t n,
                                  void *d_points, int fmt, void *stream);
 /* Powers-of-tau key of the KZG engine (Arecibo hyperkzg CommitmentKey::setup -> UniversalKZGParam::gen_srs_for_testing; the
  * primary circuit's engine on BN256, src/proof/nova.rs:65-71): d_bases_mont[i] = beta^i * g for i < n, affine Montgomery, by
  * fixed-base windows of g.  g (64 bytes affine) and beta (32 bytes, scalar field) in `fmt`; how the reference derives them from
- * the label (a seeded RNG) and the verifier key's G2 side stay on the caller's CPU. */
+ * the label (a seeded RNG) and the verifier key's G2 side stay on the caller's CPU.  Returns when the key is complete. */
 int lurk_ck_powers_dev(int curve_id, const uint8_t g[64], const uint8_t beta[32], size_t n, void *d_bases_mont, int fmt, void *stream);
 /* SHAKE256(in) -> out_len bytes (FIPS 202).  Host only (works without a GPU); the XOF behind from_label. */
 int lurk_shake256(const uint8_t *in, size_t in_len, uint8_t *out, size_t out_len);
@@ -277,7 +288,8 @@ typedef int (*lurk_challenge_fn)(void *user, int round, const uint8_t *message, 
 #define LURK_SUMCHECK_QUAD 0  /* claim = sum_i A[i] B[i]                 d_polys = {A, B}          degree 2 */
 #define LURK_SUMCHECK_CUBIC 1 /* claim = sum_i A[i] (B[i] C[i] - D[i])   d_polys = {A, B, C, D}    degree 3 */
 /* Runs all num_rounds rounds.  The polynomials are consumed (bound in place; element 0 of each ends as its final evaluation).
- * round_evals: num_rounds x (degree + 1) x 32 bytes; challenges: num_rounds x 32; final_evals: 2 or 4 x 32 (any may be NULL). */
+ * round_evals: num_rounds x (degree + 1) x 32 bytes; challenges: num_rounds x 32; final_evals: 2 or 4 x 32 (any may be NULL).
+ * Returns when done, as every call below that takes a challenge callback. */
 int lurk_sumcheck_prove_dev(int field_id, int kind, void *const *d_polys, int num_rounds, const uint8_t claim[32],
                             lurk_challenge_fn challenge, void *user, uint8_t *round_evals, uint8_t *challenges, uint8_t *final_evals,
                             int fmt, void *stream);
@@ -290,12 +302,12 @@ int lurk_sumcheck_prove_batch_dev(int field_id, int kind, int n_instances, void 
                                   const uint8_t *claims, const uint8_t *coeffs, lurk_challenge_fn challenge, void *user,
                                   uint8_t *round_evals, uint8_t *challenges, uint8_t *final_evals, int fmt, void *stream);
 /* EqPolynomial::new(tau).evals(): d_out[i] = prod_j (bit_j(i) ? tau[j] : 1 - tau[j]), tau[0] <-> the top index bit; 2^num_vars
- * elements in `fmt` (tau: host, num_vars x 32 bytes, same fmt). */
+ * elements in `fmt` (tau: host, num_vars x 32 bytes, same fmt).  Asynchronous. */
 int lurk_eq_evals_dev(int field_id, const uint8_t *tau, int num_vars, void *d_out, int fmt, void *stream);
 /* <a, b> over n Montgomery elements (MultilinearPolynomial::evaluate = <Z, eq(r)>; the c_L / c_R of an IPA round).  Synchronous. */
 int lurk_inner_product_dev(int field_id, const void *d_a, const void *d_b, size_t n, uint8_t out[32], int fmt, void *stream);
 /* one IPA folding step, in place on the first n / 2 slots: a[i] <- x a[i] + y a[i + n/2];  G[i] <- x G[i] + y G[i + n/2]
- * (CommitmentKey::fold; bases affine Montgomery; x, y host scalars in `fmt`). */
+ * (CommitmentKey::fold; bases affine Montgomery; x, y host scalars in `fmt`).  Both asynchronous. */
 int lurk_ipa_fold_scalars_dev(int field_id, void *d_a, size_t n, const uint8_t x[32], const uint8_t y[32], int fmt, void *stream);
 int lurk_ipa_fold_bases_dev(int curve_id, void *d_bases_mont, size_t n, const uint8_t x[32], const uint8_t y[32], int fmt, void *stream);
 /* All log_n rounds of InnerProductArgument::prove on device-resident a, b (2^log_n scalars each, Montgomery, consumed) under the
@@ -402,13 +414,14 @@ typedef struct lurk_spartan_proof {
  * the call returns when the proof is complete. */
 int lurk_spartan_prove_dev(lurk_spartan_ctx *ctx, const void *d_z, const void *d_E, lurk_spartan_challenge_fn challenge, void *user,
                            lurk_spartan_proof *out, void *d_joint, int fmt, void *stream);
-/* BatchedRelaxedR1CSSNARK::prove over n (1..30) running instances, instance i of shape ctxs[i] (shapes may differ; one field). */
+/* BatchedRelaxedR1CSSNARK::prove over n (1..30) running instances, instance i of shape ctxs[i] (shapes may differ; one field).  Returns when
+ * the proof is complete. */
 int lurk_spartan_prove_batch_dev(int n, lurk_spartan_ctx *const *ctxs, const void *const *d_z, const void *const *d_E,
                                  lurk_spartan_challenge_fn challenge, void *user, lurk_spartan_proof *out, void *d_joint, int fmt,
                                  void *stream);
 /* compute_eval_table_sparse alone: d_out[j] = sum_rows eq_rx[row] (A[row][j] + r B[row][j] + r^2 C[row][j]) over the padded z's
  * columns (2 num_vars elements); d_eq_rx: 2^log_rows Montgomery elements; r: 32 bytes in `fmt`.  For callers that schedule the
- * primitives themselves. */
+ * primitives themselves.  Asynchronous. */
 int lurk_spartan_eval_table_dev(lurk_spartan_ctx *ctx, const void *d_eq_rx, const uint8_t r[32], void *d_out, int fmt, void *stream);
 /* The verifier's side (RelaxedR1CSSNARK::verify, BatchedRelaxedR1CSSNARK::verify: CompressedSNARK::verify, src/proof/nova.rs:358-373).
  * lurk_spartan_matrix_evals_dev: the multilinear extensions of A, B, C at (r_x, r_y) -- r_x: log_rows elements, r_y: log_vars + 1
@@ -533,8 +546,9 @@ typedef struct lurk_compress_proof {
 /* d_z[i] / d_E[i]: primary instance i on the device, laid out as LURK_FOLD_BUF_Z1 / LURK_FOLD_BUF_E1 hold it (read, never written);
  * comm_W[i] / comm_E[i]: its commitments (96 bytes, `fmt`); d_z2, d_E2, comm_W2, comm_E2: the secondary's.  n_primary must be the
  * number of primary contexts.  The primary proof runs on `stream`, the secondary on the context's worker stream (after the work queued
- * on `stream` so far); both host threads are joined before the call returns, errors included.  A failed callback or any other error
- * returns its code with a message naming the circuit; the context stays usable.  One call at a time per context. */
+ * on `stream` so far); both host threads are joined before the call returns, errors included: the call returns when done.  A failed
+ * callback or any other error returns its code with a message naming the circuit; the context stays usable.  One call at a time per
+ * context. */
 int lurk_compress_prove_dev(lurk_compress_ctx *ctx, int n_primary, const void *const *d_z, const void *const *d_E, const uint8_t *const *comm_W,
                             const uint8_t *const *comm_E, const void *d_z2, const void *d_E2, const uint8_t comm_W2[96], const uint8_t comm_E2[96],
                             lurk_compress_challenge_fn challenge, void *user, int flags, lurk_compress_proof *out, int fmt, void *stream);
@@ -621,7 +635,8 @@ int lurk_point_combination_batch(int curve_id, int n_groups, const uint32_t *cou
  * S5  Fold helpers on device-resident vectors (Arecibo NIFS::prove / R1CSShape::commit_T /
  *     RelaxedR1CSWitness::fold; SURVEY.md Appendix B).  All vectors Montgomery form on the device.
  * ------------------------------------------------------------------------------------------------- */
-/* out[i] = a[i] + r * b[i]  (W <- W1 + r W2, E <- E1 + r T).  r: 32 bytes host, Montgomery. out may alias a. */
+/* All four asynchronous.
+ * out[i] = a[i] + r * b[i]  (W <- W1 + r W2, E <- E1 + r T).  r: 32 bytes host, Montgomery. out may alias a. */
 int lurk_axpy_dev(int field_id, const void *d_a, const void *d_b, const uint8_t r_mont[32], size_t n, void *d_out,
                   void *stream);
 /* y = M z for a CSR matrix (row_ptr: rows+1 x u64, col: nnz x u32, val: nnz elements) */
@@ -704,6 +719,16 @@ int lurk_fold_ctx_set_ro(lurk_fold_ctx *ctx, int n_absorb, const int *kinds, int
 #define LURK_FOLD_BUF_T (-5)    /* device only: cross term of the last step                             */
 #define LURK_FOLD_BUF_Z1 (-6)   /* device only: running z = (W, u, X)                                   */
 #define LURK_FOLD_BUF_E1 (-7)   /* device only: running E                                               */
+/* When the device buffers may be read or written.  The context runs on non-blocking streams of its own and takes no stream, so a
+ * caller's stream is ordered against it only through these calls:
+ *   LURK_FOLD_BUF_Z1, _E1  after lurk_fold_ctx_collect of the step that last changed them (init_running or a fold): collect returns
+ *                          once the fold has written them, so lurk_spartan_prove_dev, lurk_compress_prove_dev or
+ *                          lurk_recursive_verify_dev may read them on any stream straight after it.
+ *   LURK_FOLD_BUF_T        after lurk_fold_ctx_collect of the stage B that computed it.
+ *   LURK_FOLD_BUF_W2       after a stage A of buffer b, only after lurk_fold_ctx_sync (collect does not cover a stage A that no
+ *                          collected step consumed).
+ *   Writes for LURK_FOLD_INPUTS_RESIDENT  must be complete, not merely queued on the caller's stream, before lurk_fold_ctx_stage_a
+ *                          (e.g. cudaStreamSynchronize of that stream), and made after the previous step of buffer b was collected. */
 int lurk_fold_ctx_host_buffer(lurk_fold_ctx *ctx, int b, int which, void **ptr, size_t *bytes);
 int lurk_fold_ctx_device_buffer(lurk_fold_ctx *ctx, int b, int which, void **d_ptr, size_t *bytes);
 /* Sharded key, one process per GPU: every rank publishes a 64-byte handle of its exchange buffer (any transport: e.g. a
@@ -735,7 +760,7 @@ typedef struct lurk_fold_result {
     int status;
     uint64_t seq;               /* exchange epoch = number of commitments finished by this context */
 } lurk_fold_result;
-/* waits for the step enqueued on buffer b (init_running or stage_b_launch) and returns its record */
+/* waits for the step enqueued on buffer b (init_running or stage_b_launch), its fold of Z1 and E1 included, and returns its record */
 int lurk_fold_ctx_collect(lurk_fold_ctx *ctx, int b, lurk_fold_result *out, int fmt);
 /* Verifier-side sanity of the running instance, computed on the device: rows with (A z) o (B z) != u (C z) + E, and
  * whether commit(W) / commit(E) recomputed from the vectors equal the folded commitments.  Synchronous. */
@@ -750,6 +775,7 @@ int lurk_fold_ctx_sync(lurk_fold_ctx *ctx);
  *     In-place length-2^log_n DFT over the field's 2-adic subgroup, natural order in and out, Montgomery form.
  *     Roots: omega = g^((p-1)/2^s) with g the multiplicative generator of halo2curves / pasta_curves.
  * ------------------------------------------------------------------------------------------------- */
+/* Asynchronous (the first transform of a size and direction on a device waits while it builds that size's twiddles). */
 int lurk_ntt_dev(int field_id, void *d_data, int log_n, int inverse, void *stream);
 
 #ifdef __cplusplus

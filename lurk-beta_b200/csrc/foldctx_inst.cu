@@ -798,6 +798,10 @@ struct FoldCtx final : FoldCtxBase {
         LURK_TRY(chk_b(b));
         if (!b_pending[b]) { set_error("buffer %d: nothing to collect", b); return LURK_ERR_ARG; }
         LURK_CUDA_TRY(cudaEventSynchronize(ev_done[b]));
+        // the record is ready once the challenge is; the running instance only once the fold on sB has written z1, E1 and A z1 .. C z1.
+        // Callers read Z1 / E1 right after collect (lurk_spartan_prove_dev, lurk_compress_prove_dev, lurk_recursive_verify_dev), on
+        // streams the context does not know.
+        LURK_CUDA_TRY(cudaEventSynchronize(ev_fold[b]));
         b_pending[b] = false;
         const Rec &r = *h_rec[b];
         if (out) {
