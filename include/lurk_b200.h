@@ -148,6 +148,41 @@ int lurk_trie_witness_batch_dev(int field_id, int op, int height, const void *d_
 int lurk_trie_witness_scatter_dev(int field_id, int op, int height, const void *d_inputs, size_t count, const uint64_t *d_offsets,
                                   void *d_W, int fmt, void *stream);
 
+/* Device-resident trie node store (the reference's Trie over its inverse Poseidon cache, arity 8, height H = 1..
+ * LURK_TRIE_MAX_HEIGHT): content-addressed nodes, digest -> 8-element preimage, only ever added.  Creation registers the
+ * H empty roots; on a machine without a GPU the context is created without a store and every call that needs one returns
+ * LURK_ERR_NOGPU.  capacity_nodes bounds the node count (H .. 2^31 - 1); the store takes about 300 bytes per node.
+ * One context is used by one thread at a time; separate contexts may run on separate threads. */
+typedef struct lurk_trie_ctx lurk_trie_ctx;
+int lurk_trie_ctx_create(int field_id, int height, uint64_t capacity_nodes, lurk_trie_ctx **out);
+void lurk_trie_ctx_destroy(lurk_trie_ctx *ctx);
+/* the root of the empty trie of height H, in fmt */
+int lurk_trie_ctx_empty_root(lurk_trie_ctx *ctx, uint8_t out[32], int fmt);
+int lurk_trie_ctx_info(const lurk_trie_ctx *ctx, uint64_t *node_count, uint64_t *capacity);
+/* Add n existing nodes (preimages: n x 8 elements in fmt, e.g. a host inverse cache), hashed on the GPU; their digests
+ * go to digests_out (n elements in fmt, may be NULL).  A node already stored is not added again.  Returns when done. */
+int lurk_trie_ctx_register(lurk_trie_ctx *ctx, const uint8_t *preimages, size_t n, uint8_t *digests_out, int fmt);
+/* Apply n operations in program order, exactly as the reference's sequential Trie would.  Operation i: kinds[i]
+ * LURK_TRIE_LOOKUP or LURK_TRIE_INSERT, keys[i], values[i] (read for inserts only), and its root: prev[i] = -1 names
+ * roots[i], which must be stored; prev[i] = j < i names the root insert j of this batch produced.  An insert with prev =
+ * j continues j's chain and j must be that chain's latest insert (no forks inside a batch; each insert with prev = -1
+ * starts its own chain, forks from a stored root are fine); a lookup may name any earlier insert and reads that version.
+ * A key's path is its low 3H bits, most significant 3-bit chunk first.  Arrays are host memory of n entries (elements
+ * 32 bytes in fmt); roots[i] is read only where prev[i] = -1 and values[i] only for an insert, so roots may be NULL
+ * when every prev[i] >= 0 and values when the batch has no insert.
+ * results_out (n elements in fmt, may be NULL): a lookup's value (0 when absent), an insert's new root.  The proofs go
+ * to device memory in fmt, in lurk_trie_witness_batch's input layout: the lookups' in their program order to
+ * d_lookup_inputs (2 + 8H elements each), the inserts' to d_insert_inputs (3 + 16H each); either may be NULL.  New nodes
+ * are registered, so later batches may start from any root produced.
+ * Refused before any launch, with the operation's index in lurk_last_error(), as LURK_ERR_ARG: a bad kind or prev, a
+ * fork, an element >= p, a NULL roots or values array that is read, node count + H x inserts > capacity (naming the
+ * first insert that would not fit).  Then
+ * LURK_ERR_NOGPU.  A root or node missing from the store (the reference's MissingPreimage) returns LURK_ERR_RANGE naming
+ * the first such operation and the digest; the store, the node count and the outputs are then left as they were.
+ * Ordered on `stream` after the caller's earlier work there; returns when the batch is applied. */
+int lurk_trie_ctx_apply(lurk_trie_ctx *ctx, size_t n, const int *kinds, const int64_t *prev, const uint8_t *roots, const uint8_t *keys,
+                        const uint8_t *values, int fmt, uint8_t *results_out, void *d_lookup_inputs, void *d_insert_inputs, void *stream);
+
 /* ---------------------------------------------------------------------------------------------------
  * S2  DAG hydration.  Replaces StoreCore::hydrate_z_cache / hash_ptr_val_unsafe (src/lem/store_core.rs:199-269)
  *     with the preimage layouts of `impl StoreHasher for PoseidonCache` (src/lem/store.rs:29-78).

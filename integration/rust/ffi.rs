@@ -44,6 +44,8 @@ pub const LURK_SPARTAN_BATCH_EVAL: c_int = 5;
 pub const LURK_SPARTAN_PCS: c_int = 6;
 #[repr(C)]
 pub struct lurk_compress_ctx { _private: [u8; 0] }
+#[repr(C)]
+pub struct lurk_trie_ctx { _private: [u8; 0] }
 pub const LURK_PCS_HYPERKZG: c_int = 0;
 pub const LURK_PCS_IPA: c_int = 1;
 pub const LURK_COMPRESS_SEQUENTIAL: c_int = 1;
@@ -120,6 +122,16 @@ extern "C" {
                                        stream: *mut c_void) -> c_int;
     pub fn lurk_trie_witness_scatter_dev(field_id: c_int, op: c_int, height: c_int, d_inputs: *const c_void, count: usize, d_offsets: *const u64,
                                          d_w: *mut c_void, fmt: c_int, stream: *mut c_void) -> c_int;
+    // a12 -- the trie's own operations (Trie::prove_lookup / prove_insert over the inverse Poseidon cache, mod.rs:718-811) on a
+    // device node store; the replay of a proved evaluation's trie calls hands (op, root, key, value) instead of packed proofs
+    pub fn lurk_trie_ctx_create(field_id: c_int, height: c_int, capacity_nodes: u64, out: *mut *mut lurk_trie_ctx) -> c_int;
+    pub fn lurk_trie_ctx_destroy(ctx: *mut lurk_trie_ctx);
+    pub fn lurk_trie_ctx_empty_root(ctx: *mut lurk_trie_ctx, out: *mut u8, fmt: c_int) -> c_int;
+    pub fn lurk_trie_ctx_info(ctx: *const lurk_trie_ctx, node_count: *mut u64, capacity: *mut u64) -> c_int;
+    pub fn lurk_trie_ctx_register(ctx: *mut lurk_trie_ctx, preimages: *const u8, n: usize, digests_out: *mut u8, fmt: c_int) -> c_int;
+    pub fn lurk_trie_ctx_apply(ctx: *mut lurk_trie_ctx, n: usize, kinds: *const c_int, prev: *const i64, roots: *const u8, keys: *const u8,
+                               values: *const u8, fmt: c_int, results_out: *mut u8, d_lookup_inputs: *mut c_void, d_insert_inputs: *mut c_void,
+                               stream: *mut c_void) -> c_int;
     // S2 -- StoreCore::hydrate_z_cache (src/lem/store_core.rs:256-269)
     pub fn lurk_dag_hash(field_id: c_int, nodes: *const lurk_dag_node, n: usize, atom_digests: *const u8, n_atoms: usize, out: *mut u8) -> c_int;
     // S4 -- Arecibo CommitmentEngineTrait::commit (call sites src/proof/nova.rs:287,292)

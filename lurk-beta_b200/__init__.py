@@ -17,8 +17,8 @@ from .hash import HashConstants, PoseidonCache
 from .sha256 import Sha256Coprocessor, sha256_witness_batch, witness_block
 from .slots import SlotType, compute_witness_size, generate_slots_witnesses, slot_witness_batch_bytes
 from .store import StoreCore
-from .trie import (TRIE_INSERT, TRIE_LOOKUP, InsertProof, LookupProof, StandardTrie, Trie, insert_inputs, lookup_inputs,
-                   trie_witness_batch, trie_witness_block)
+from .trie import (TRIE_INSERT, TRIE_LOOKUP, DeviceTrie, InsertProof, LookupProof, StandardTrie, Trie, insert_inputs, lookup_inputs,
+                   trie_witness_batch, trie_witness_block, write_trie_batch)
 
 __all__ = [
     "CommitmentKey", "ShardedCommitmentKey", "NovaFoldContext", "SuperNovaFoldContext", "point_sum", "shard_bounds", "synthetic_bases", "ck_size", "from_label",
@@ -26,7 +26,8 @@ __all__ = [
     "hash_to_curve_batch", "shake256", "spartan", "HashConstants", "PoseidonCache", "SlotType",
     "compute_witness_size", "generate_slots_witnesses", "slot_witness_batch_bytes",
     "Sha256Coprocessor", "sha256_witness_batch", "witness_block", "StoreCore", "StandardTrie", "Trie", "LookupProof",
-    "InsertProof", "TRIE_LOOKUP", "TRIE_INSERT", "lookup_inputs", "insert_inputs", "trie_witness_block", "trie_witness_batch", "LurkError",
+    "InsertProof", "TRIE_LOOKUP", "TRIE_INSERT", "lookup_inputs", "insert_inputs", "trie_witness_block", "trie_witness_batch", "DeviceTrie",
+    "write_trie_batch", "LurkError",
     "FIELD_BN254_FR", "FIELD_BN254_FQ", "FIELD_PALLAS_FQ", "FIELD_PALLAS_FP", "CURVE_BN254_G1", "CURVE_GRUMPKIN",
     "CURVE_PALLAS", "CURVE_VESTA", "FMT_CANONICAL", "FMT_MONTGOMERY",
 ]

@@ -131,6 +131,12 @@ PROTOTYPES = {
     "lurk_trie_witness_batch": (_i, [_i, _i, _i, _vp, _sz, _vp, _i]),
     "lurk_trie_witness_batch_dev": (_i, [_i, _i, _i, _vp, _sz, _vp, _i, _vp]),
     "lurk_trie_witness_scatter_dev": (_i, [_i, _i, _i, _vp, _sz, _vp, _vp, _i, _vp]),
+    "lurk_trie_ctx_create": (_i, [_i, _i, C.c_uint64, C.POINTER(_vp)]),
+    "lurk_trie_ctx_destroy": (None, [_vp]),
+    "lurk_trie_ctx_empty_root": (_i, [_vp, _vp, _i]),
+    "lurk_trie_ctx_info": (_i, [_vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "lurk_trie_ctx_register": (_i, [_vp, _vp, _sz, _vp, _i]),
+    "lurk_trie_ctx_apply": (_i, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "lurk_dag_hash": (_i, [_i, _vp, _sz, _vp, _sz, _vp]),
     "lurk_dag_hash_plan": (_i, [_vp, _sz, _sz, C.POINTER(DagPlan)]),
     "lurk_msm_ctx_create": (_i, [_i, _vp, _sz, _i, C.POINTER(_vp)]),

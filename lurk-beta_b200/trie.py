@@ -12,6 +12,7 @@ The lookup and insert circuits' whole aux blocks (synthesize_lookup_aux, mod.rs:
 226-268) are written on the GPU from the calls' proofs (`prove_lookup` / `prove_insert`, mod.rs:718-776):
 `lookup_inputs` / `insert_inputs` pack a call, `trie_witness_batch` writes the blocks (include/lurk_b200.h,
 lurk_trie_witness_*), and the fold context writes them straight into W (NovaFoldContext.add_trie_batch)."""
+import ctypes as C
 from collections import namedtuple
 
 import numpy as np
@@ -19,7 +20,7 @@ import numpy as np
 from . import _capi
 from .hash import PoseidonCache
 from .slots import SlotType, slot_witness_batch_bytes
-from .field import pack
+from .field import pack, unpack
 
 TRIE_LOOKUP, TRIE_INSERT = _capi.TRIE_LOOKUP, _capi.TRIE_INSERT
 LookupProof = namedtuple("LookupProof", "preimage_path")            # root level first, ARITY elements each
@@ -152,3 +153,118 @@ def trie_witness_batch(field_id, op, height, inputs, fmt=_capi.FMT_CANONICAL):
     out = np.zeros(count * blk * 32, dtype=np.uint8)
     _capi.check(_capi.lib().lurk_trie_witness_batch(field_id, op, height, _capi.np_ptr(src), count, _capi.np_ptr(out), fmt))
     return out
+
+
+class DeviceTrie:
+    """A trie node store on the GPU (include/lurk_b200.h, lurk_trie_ctx_*): arity 8, height 1..85, one field.  `apply`
+    runs a batch of lookups and inserts in program order, exactly as the sequential `Trie` would, and writes every
+    call's proof in `lookup_inputs` / `insert_inputs` layout to device memory, ready for the witness kernels."""
+
+    def __init__(self, field_id=_capi.FIELD_BN254_FR, height=85, capacity=1 << 20):
+        self.field_id, self.height = field_id, height
+        self._lib = _capi.lib()
+        ctx = C.c_void_p()
+        _capi.check(self._lib.lurk_trie_ctx_create(field_id, height, capacity, C.byref(ctx)))
+        self._ctx = ctx
+
+    def close(self):
+        if self._ctx:
+            self._lib.lurk_trie_ctx_destroy(self._ctx)
+            self._ctx = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def empty_root(self, fmt=_capi.FMT_CANONICAL):
+        out = np.zeros(32, dtype=np.uint8)
+        _capi.check(self._lib.lurk_trie_ctx_empty_root(self._ctx, _capi.np_ptr(out), fmt))
+        return unpack(out)[0]
+
+    @property
+    def node_count(self):
+        n, cap = C.c_uint64(), C.c_uint64()
+        _capi.check(self._lib.lurk_trie_ctx_info(self._ctx, C.byref(n), C.byref(cap)))
+        return n.value
+
+    @property
+    def capacity(self):
+        n, cap = C.c_uint64(), C.c_uint64()
+        _capi.check(self._lib.lurk_trie_ctx_info(self._ctx, C.byref(n), C.byref(cap)))
+        return cap.value
+
+    def register(self, preimages, fmt=_capi.FMT_CANONICAL):
+        """add existing nodes (8-tuples of ints, e.g. a host `Trie`'s inverse cache values) -> their digests"""
+        pre = pack([int(x) for p in preimages for x in p])
+        if pre.size % (32 * 8):
+            raise ValueError("preimages must have 8 elements each")
+        n = pre.size // (32 * 8)
+        out = np.zeros(n * 32, dtype=np.uint8)
+        _capi.check(self._lib.lurk_trie_ctx_register(self._ctx, _capi.np_ptr(pre), n, _capi.np_ptr(out), fmt))
+        return unpack(out)
+
+    def apply(self, ops, fmt=_capi.FMT_CANONICAL, lookup_out=None, insert_out=None, stream=None):
+        """ops: sequence of (kind, prev, root, key, value), ints (root read where prev = -1, value for inserts).
+        Returns (results, lookup_inputs, insert_inputs): results a list of ints (lookup: the value, 0 when absent;
+        insert: the new root), the proofs as uint8 CUDA tensors of (lookups, 2 + 8H, 32) and (inserts, 3 + 16H, 32)
+        elements in fmt.  lookup_out / insert_out: device buffers (torch tensors) to write the proofs into instead."""
+        import torch
+        n = len(ops)
+        kinds = np.array([o[0] for o in ops], dtype=np.int32)
+        prev = np.array([o[1] for o in ops], dtype=np.int64)
+        roots, keys, vals = (pack([int(o[k]) for o in ops]) if n else np.zeros(0, dtype=np.uint8) for k in (2, 3, 4))
+        n_ins = int((kinds == TRIE_INSERT).sum())
+        H = self.height
+        if lookup_out is None:
+            lookup_out = torch.empty((n - n_ins, trie_n_inputs(TRIE_LOOKUP, H), 32), dtype=torch.uint8, device="cuda")
+        if insert_out is None:
+            insert_out = torch.empty((n_ins, trie_n_inputs(TRIE_INSERT, H), 32), dtype=torch.uint8, device="cuda")
+        for out, op, count in ((lookup_out, TRIE_LOOKUP, n - n_ins), (insert_out, TRIE_INSERT, n_ins)):
+            want = count * trie_n_inputs(op, H) * 32
+            if out.dtype != torch.uint8 or not out.is_cuda or not out.is_contiguous() or out.numel() != want:
+                raise ValueError(f"the {'lookup' if op == TRIE_LOOKUP else 'insert'} proofs need a contiguous uint8 CUDA tensor of "
+                                 f"{want} bytes, not {out.dtype} on {out.device} with {out.numel()} elements")
+        res = np.zeros(n * 32, dtype=np.uint8)
+        if stream is None:
+            stream = torch.cuda.current_stream().cuda_stream
+        _capi.check(self._lib.lurk_trie_ctx_apply(self._ctx, n, _capi.np_ptr(kinds), _capi.np_ptr(prev), _capi.np_ptr(roots), _capi.np_ptr(keys),
+                                                  _capi.np_ptr(vals), fmt, _capi.np_ptr(res), lookup_out.data_ptr() if lookup_out.numel() else None,
+                                                  insert_out.data_ptr() if insert_out.numel() else None, stream))
+        return unpack(res), lookup_out, insert_out
+
+
+def write_trie_batch(device_trie, fold_ctx, b, batch_index, ops):
+    """apply `ops` (all lookups or all inserts, the op of the NovaFoldContext's trie batch `batch_index`; for a
+    SuperNovaFoldContext pass the circuit's context, `contexts[i]`) and write their proofs, Montgomery form, straight
+    into the batch's device buffer of buffer set b, for stage_a(b, resident=True).  ops as for DeviceTrie.apply, in
+    canonical ints; returns the results as canonical ints."""
+    import torch
+    kinds = {int(o[0]) for o in ops}
+    if len(kinds) > 1:
+        raise ValueError("a trie batch holds calls of one op")
+    op = kinds.pop() if kinds else TRIE_LOOKUP
+    # the library refuses elements >= p; here they must be refused before the conversion reduces them
+    p = int.from_bytes(_modulus(device_trie.field_id), "little")
+    for i, (_, prev, root, key, value) in enumerate(ops):
+        for name, x, read in (("root", root, prev < 0), ("key", key, True), ("value", value, op == TRIE_INSERT)):
+            if read and not 0 <= int(x) < p:
+                raise ValueError(f"trie operation {i}: the {name} is not reduced below the field modulus")
+    view = fold_ctx.device_view(b, batch_index)
+    per = trie_n_inputs(op, device_trie.height) * 32
+    if view.numel() != per * len(ops):
+        raise ValueError(f"the batch's device buffer holds {view.numel() // per} calls, not {len(ops)}")
+    out = view.view(len(ops), -1, 32)
+    empty = torch.empty((0, 1, 32), dtype=torch.uint8, device="cuda")
+    r_mont, r_inv = (1 << 256) % p, pow(1 << 256, -1, p)
+    mont = [(k, prev, int(root) * r_mont % p, int(key) * r_mont % p, int(value) * r_mont % p) for k, prev, root, key, value in ops]
+    res, _, _ = device_trie.apply(mont, fmt=_capi.FMT_MONTGOMERY, lookup_out=out if op == TRIE_LOOKUP else empty,
+                                  insert_out=out if op == TRIE_INSERT else empty)
+    return [r * r_inv % p for r in res]
+
+
+def _modulus(field_id):
+    out = np.zeros(32, dtype=np.uint8)
+    _capi.check(_capi.lib().lurk_field_modulus(field_id, _capi.np_ptr(out)))
+    return out.tobytes()
