@@ -182,6 +182,25 @@ int lurk_trie_ctx_register(lurk_trie_ctx *ctx, const uint8_t *preimages, size_t 
  * Ordered on `stream` after the caller's earlier work there; returns when the batch is applied. */
 int lurk_trie_ctx_apply(lurk_trie_ctx *ctx, size_t n, const int *kinds, const int64_t *prev, const uint8_t *roots, const uint8_t *keys,
                         const uint8_t *values, int fmt, uint8_t *results_out, void *d_lookup_inputs, void *d_insert_inputs, void *stream);
+/* Device-resident forms, for operations and preimages already in device memory (e.g. a replay batch uploaded in one copy).
+ * lurk_trie_ctx_apply_dev: lurk_trie_ctx_apply with every array in device memory -- d_kinds (int32), d_prev (int64),
+ * d_roots / d_keys / d_values (n elements in fmt; d_roots and d_values may be NULL when never read), d_results (n elements
+ * in fmt, may be NULL) -- and the batch planned on the GPU instead of the host.  The proof buffers are sized by the
+ * caller, as for lurk_trie_ctx_apply.  Refused on the host, as LURK_ERR_ARG and in this order, before LURK_ERR_NOGPU: a
+ * null ctx, a bad fmt, NULL d_kinds, d_prev or d_keys with n > 0, n >= 2^31.  Every other refusal is found on the device
+ * and returns the code lurk_trie_ctx_apply returns on the same arrays, naming the same operation: a bad kind or prev, a
+ * prev naming a lookup, a fork, an element >= p, a NULL d_roots or d_values that would be read, the capacity (the first
+ * insert that does not fit), MissingPreimage (LURK_ERR_RANGE, with the digest).  On any refusal the store, the node count,
+ * d_results and the proof buffers are left as they were.
+ * lurk_trie_ctx_register_dev: lurk_trie_ctx_register with d_preimages (n x 8 elements in fmt) and d_digests_out (n in
+ * fmt, may be NULL) in device memory.  Refused on the host as LURK_ERR_ARG, in this order and before LURK_ERR_NOGPU: a
+ * null ctx, a bad fmt, NULL d_preimages with n > 0, n over the remaining capacity; an element >= p is found on the device
+ * and refused as LURK_ERR_ARG naming the preimage and the element.
+ * Both are ordered on `stream` after the caller's earlier work there and return when the batch is applied (so the error
+ * is exact); neither returns before its device work is done. */
+int lurk_trie_ctx_apply_dev(lurk_trie_ctx *ctx, size_t n, const int32_t *d_kinds, const int64_t *d_prev, const void *d_roots, const void *d_keys,
+                            const void *d_values, int fmt, void *d_results, void *d_lookup_inputs, void *d_insert_inputs, void *stream);
+int lurk_trie_ctx_register_dev(lurk_trie_ctx *ctx, const void *d_preimages, size_t n, void *d_digests_out, int fmt, void *stream);
 
 /* ---------------------------------------------------------------------------------------------------
  * S2  DAG hydration.  Replaces StoreCore::hydrate_z_cache / hash_ptr_val_unsafe (src/lem/store_core.rs:199-269)

@@ -132,6 +132,12 @@ extern "C" {
     pub fn lurk_trie_ctx_apply(ctx: *mut lurk_trie_ctx, n: usize, kinds: *const c_int, prev: *const i64, roots: *const u8, keys: *const u8,
                                values: *const u8, fmt: c_int, results_out: *mut u8, d_lookup_inputs: *mut c_void, d_insert_inputs: *mut c_void,
                                stream: *mut c_void) -> c_int;
+    // the same on operations already in device memory: a shim may upload a replay batch in one copy and plan it on the GPU
+    pub fn lurk_trie_ctx_apply_dev(ctx: *mut lurk_trie_ctx, n: usize, d_kinds: *const i32, d_prev: *const i64, d_roots: *const c_void,
+                                   d_keys: *const c_void, d_values: *const c_void, fmt: c_int, d_results: *mut c_void, d_lookup_inputs: *mut c_void,
+                                   d_insert_inputs: *mut c_void, stream: *mut c_void) -> c_int;
+    pub fn lurk_trie_ctx_register_dev(ctx: *mut lurk_trie_ctx, d_preimages: *const c_void, n: usize, d_digests_out: *mut c_void, fmt: c_int,
+                                      stream: *mut c_void) -> c_int;
     // S2 -- StoreCore::hydrate_z_cache (src/lem/store_core.rs:256-269)
     pub fn lurk_dag_hash(field_id: c_int, nodes: *const lurk_dag_node, n: usize, atom_digests: *const u8, n_atoms: usize, out: *mut u8) -> c_int;
     // S4 -- Arecibo CommitmentEngineTrait::commit (call sites src/proof/nova.rs:287,292)

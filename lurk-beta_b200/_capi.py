@@ -137,6 +137,8 @@ PROTOTYPES = {
     "lurk_trie_ctx_info": (_i, [_vp, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "lurk_trie_ctx_register": (_i, [_vp, _vp, _sz, _vp, _i]),
     "lurk_trie_ctx_apply": (_i, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "lurk_trie_ctx_apply_dev": (_i, [_vp, _sz, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "lurk_trie_ctx_register_dev": (_i, [_vp, _vp, _sz, _vp, _i, _vp]),
     "lurk_dag_hash": (_i, [_i, _vp, _sz, _vp, _sz, _vp]),
     "lurk_dag_hash_plan": (_i, [_vp, _sz, _sz, C.POINTER(DagPlan)]),
     "lurk_msm_ctx_create": (_i, [_i, _vp, _sz, _i, C.POINTER(_vp)]),

@@ -18,7 +18,10 @@
 //               launch of poseidon_kernel.cuh) and registered.  Nothing in one level depends on another thread's work
 //               in the same level, and no level waits for the host.
 //   3. finish   roots, keys, values and results.
-// The host only checks the arguments, sorts the inserts by (chain, key path) once, and waits for the end of the batch.
+// lurk_trie_ctx_apply plans on the host (plan_batch: argument checks, chains, ranks, the inserts sorted by (chain, key
+// path) once) and uploads the plan.  lurk_trie_ctx_apply_dev, whose operations are already in device memory, plans on
+// the device (plan_dev: validate, pointer jumping over prev, a CUB scan for the ranks, stable CUB radix passes for the
+// order) and reads back only a status word before the levels.  Both then run the same levels (run_levels).
 #include "common.cuh"
 #include "poseidon_api.h"
 #include "trie.cuh"
@@ -235,6 +238,136 @@ __global__ void fill8_kernel(uint8_t *pre, const uint8_t *d) {
     if (i < ARITY * 32) pre[i] = d[i & 31];
 }
 
+// ---- planning on the device (lurk_trie_ctx_apply_dev): the same OpDev array, bases, canonical keys and values, insert
+// order and lcp that plan_batch builds on the host.  Per-operation refusals go into one 64-bit word as (i << 8) | code,
+// the lowest operation winning, and the codes of one operation in the order plan_batch checks them.
+enum PlanErr : unsigned { PE_KIND = 1, PE_PREV, PE_PREV_LOOKUP, PE_FORK, PE_ROOTS_NULL, PE_VALUES_NULL, PE_ROOT, PE_KEY, PE_VALUE };
+
+struct PlanStatus {
+    unsigned long long err;
+    uint32_t inserts, cap_first;   // m, and the operation of insert rank `fits` (NONE: there is none)
+};
+
+// first[j]: the lowest insert with prev = j.  Once every earlier operation is valid the inserts of a chain form a list,
+// so an insert i with prev = j is plan_batch's fork (latest[chain] != j) exactly when first[j] != i.
+__global__ void first_continuer_kernel(int n, const int32_t *__restrict__ kinds, const int64_t *__restrict__ prev, uint32_t *first) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int64_t j = prev[i];
+    if (kinds[i] == LURK_TRIE_INSERT && j >= 0 && j < i) atomicMin(first + j, (uint32_t)i);
+}
+
+// one operation: checks, canonical key / value / root, masked path, bound; link[i] = a valid prev, else i (the chain's
+// head after pointer jumping); flags[i] = 1 for an insert
+template <class F>
+__global__ void __launch_bounds__(TS_THREADS) validate_kernel(int n, int height, const int32_t *__restrict__ kinds, const int64_t *__restrict__ prev,
+                                                              const F *__restrict__ roots, const F *__restrict__ keys_in, const F *__restrict__ vals_in,
+                                                              int fmt, const uint32_t *__restrict__ first, OpDev *__restrict__ ops, F *__restrict__ base,
+                                                              F *__restrict__ keys, F *__restrict__ vals, uint32_t *__restrict__ link,
+                                                              uint32_t *__restrict__ flags, PlanStatus *status) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int k = kinds[i];
+    const int64_t j = prev[i];
+    const bool ins = k == LURK_TRIE_INSERT;
+    link[i] = j >= 0 && j < i ? (uint32_t)j : (uint32_t)i;
+    flags[i] = ins;
+    unsigned code = 0;
+    F root = F::zero(), key = F::zero(), val = F::zero();
+    if (k != LURK_TRIE_LOOKUP && !ins) code = PE_KIND;
+    else if (j < -1 || j >= i) code = PE_PREV;
+    else if (j >= 0 && kinds[j] != LURK_TRIE_INSERT) code = PE_PREV_LOOKUP;
+    else if (ins && j >= 0 && first[j] != (uint32_t)i) code = PE_FORK;
+    else if (j < 0 && !roots) code = PE_ROOTS_NULL;
+    else if (ins && !vals_in) code = PE_VALUES_NULL;
+    else {
+        if (j < 0) root = load_fe<F>(roots + i);
+        key = load_fe<F>(keys_in + i);
+        if (ins) val = load_fe<F>(vals_in + i);
+        if (j < 0 && !root.is_reduced()) code = PE_ROOT;
+        else if (!key.is_reduced()) code = PE_KEY;
+        else if (!val.is_reduced()) code = PE_VALUE;
+    }
+    if (code) { atomicMin(&status->err, ((unsigned long long)i << 8) | code); return; }
+    if (fmt == LURK_FMT_MONTGOMERY) { root = root.to_canonical(); key = key.to_canonical(); val = val.to_canonical(); }
+    OpDev o{};
+    o.kind = (uint32_t)k;
+    o.prev = (int32_t)j;
+    o.bound = ins ? i - 1 : (int32_t)j;
+    const int bits = 3 * height;   // the path is the key's low 3H bits
+#pragma unroll
+    for (int w = 0; w < 8; w++) {
+        const int lo = 32 * w;
+        o.path[w] = lo >= bits ? 0u : (bits - lo < 32 ? key.v[w] & ((1u << (bits - lo)) - 1) : key.v[w]);
+    }
+    ops[i] = o;   // chain and rank follow in chain_rank_kernel
+    store_fe(base + i, root);
+    store_fe(keys + i, key);
+    store_fe(vals + i, val);
+}
+
+// one round of pointer jumping over prev
+__global__ void jump_kernel(int n, const uint32_t *__restrict__ in, uint32_t *__restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = in[in[i]];
+}
+
+// chain, base root from the chain's head, rank (incl: inclusive scan of the insert flags); the inserts in index order
+// go to order[rank].  Nothing is planned further once an operation is refused.
+template <class F>
+__global__ void __launch_bounds__(TS_THREADS) chain_rank_kernel(int n, const uint32_t *__restrict__ head, const uint32_t *__restrict__ incl,
+                                                                uint64_t fits, OpDev *ops, F *base, uint32_t *__restrict__ order,
+                                                                PlanStatus *status) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || status->err != NO_ERR) return;
+    OpDev &o = ops[i];
+    const uint32_t c = head[i];
+    o.chain = c;
+    if (o.prev >= 0) store_fe(base + i, load_fe<F>(base + c));   // a chain's head has prev = -1 and is not written here
+    if (o.kind == LURK_TRIE_INSERT) {
+        o.rank = incl[i] - 1;
+        order[o.rank] = (uint32_t)i;
+        if (o.rank == fits) status->cap_first = (uint32_t)i;
+    } else {
+        o.rank = (uint32_t)i - incl[i];
+    }
+    if (i == n - 1) status->inserts = incl[i];
+}
+
+// the sort key of one least-significant-first pass: path word w (0..7), then the chain (w = 8)
+__global__ void order_key_kernel(int m, const OpDev *__restrict__ ops, const uint32_t *__restrict__ order, int w, uint32_t *__restrict__ key) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= m) return;
+    const OpDev &o = ops[order[p]];
+    key[p] = w < 8 ? o.path[w] : o.chain;
+}
+
+// plan_batch's lcp: common leading chunks of order[p - 1] and order[p], -1 across chains
+__global__ void lcp_kernel(int m, int height, const OpDev *__restrict__ ops, const uint32_t *__restrict__ order, int16_t *__restrict__ lcp) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= m) return;
+    if (p == 0) { lcp[0] = 0; return; }
+    const OpDev &a = ops[order[p - 1]], &b = ops[order[p]];
+    if (a.chain != b.chain) { lcp[p] = -1; return; }
+    int hi = -1;   // the highest differing bit
+    for (int w = 7; w >= 0 && hi < 0; w--) {
+        const uint32_t x = a.path[w] ^ b.path[w];
+        if (x) hi = 32 * w + 31 - __clz(x);
+    }
+    lcp[p] = (int16_t)(hi < 0 ? height : height - 1 - hi / 3);
+}
+
+// register_dev's input: canonical preimages, and the lowest unreduced element's index in *bad
+template <class F>
+__global__ void __launch_bounds__(TS_THREADS) canon_check_kernel(size_t n, const F *__restrict__ in, int fmt, F *__restrict__ out,
+                                                                 unsigned long long *bad) {
+    const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const F x = load_fe<F>(in + e);
+    if (!x.is_reduced()) { atomicMin(bad, (unsigned long long)e); return; }
+    store_fe(out + e, fmt == LURK_FMT_MONTGOMERY ? x.to_canonical() : x);
+}
+
 unsigned blocks(size_t n) { return (unsigned)((n + TS_THREADS - 1) / TS_THREADS); }
 
 // a 256-byte aligned bump allocator over one device buffer
@@ -278,7 +411,7 @@ struct lurk_trie_ctx {
     uint64_t capacity, count = 0, mask = 0;
     int device = -1;
     uint8_t empty_root[32] = {};
-    DevBuf table, dig, pre, dcount, err, scratch;
+    DevBuf table, dig, pre, dcount, err, plan, scratch;   // plan: one batch's plan (and its planner's scratch); scratch: its levels
 };
 
 namespace lurk {
@@ -305,10 +438,10 @@ int sync_count(lurk_trie_ctx *ctx, cudaStream_t st) {
     return LURK_OK;
 }
 
-int ensure_scratch(lurk_trie_ctx *ctx, size_t bytes) {
-    if (ctx->scratch.bytes >= bytes) return LURK_OK;
-    LURK_CUDA_TRY(cudaDeviceSynchronize());   // the old scratch may still be read by an earlier call's stream
-    return ctx->scratch.alloc(bytes);
+int ensure(DevBuf &b, size_t bytes) {
+    if (b.bytes >= bytes) return LURK_OK;
+    LURK_CUDA_TRY(cudaDeviceSynchronize());   // the old buffer may still be read by an earlier call's stream
+    return b.alloc(bytes);
 }
 
 template <class F>
@@ -439,9 +572,131 @@ int plan_batch(const lurk_trie_ctx *ctx, size_t n, const int *kinds, const int64
     return LURK_OK;
 }
 
+// one batch's plan in device memory: the host planner's upload or the device planner's output.  order and lcp hold the
+// m inserts; the rest of the arrays n entries.  The device planner's own scratch follows them.
 template <class F>
-int apply_batch(lurk_trie_ctx *ctx, const Plan &P, uint8_t *results_out, void *d_lookup, void *d_insert, int fmt, cudaStream_t st) {
-    const int n = (int)P.ops.size(), m = P.inserts, H = ctx->height;
+struct DevPlan {
+    OpDev *ops;
+    F *base, *keys, *vals;
+    uint32_t *order;
+    int16_t *lcp;
+    uint32_t *first, *link_a, *link_b, *flags, *incl, *key_a, *key_b, *order_b;
+    PlanStatus *status;
+    void *tmp;
+    size_t tmp_bytes = 0;
+};
+
+template <class F>
+int take_plan(lurk_trie_ctx *ctx, int n, bool planner, cudaStream_t st, DevPlan<F> &D) {
+    if (planner) {   // CUB scratch for one scan of n flags and one stable 32-bit key-value sort of up to n inserts
+        size_t scan_bytes = 0, sort_bytes = 0;
+        cub::DoubleBuffer<uint32_t> k(nullptr, nullptr), v(nullptr, nullptr);
+        LURK_CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr, n, st));
+        LURK_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, k, v, n, 0, 32, st));
+        D.tmp_bytes = std::max(scan_bytes, sort_bytes);
+    }
+    auto lay = [&](Carve &c) {
+        D.ops = c.take<OpDev>(n); D.base = c.take<F>(n); D.keys = c.take<F>(n); D.vals = c.take<F>(n);
+        D.order = c.take<uint32_t>(n); D.lcp = c.take<int16_t>(n);
+        if (!planner) return;
+        D.first = c.take<uint32_t>(n); D.link_a = c.take<uint32_t>(n); D.link_b = c.take<uint32_t>(n); D.flags = c.take<uint32_t>(n);
+        D.incl = c.take<uint32_t>(n); D.key_a = c.take<uint32_t>(n); D.key_b = c.take<uint32_t>(n); D.order_b = c.take<uint32_t>(n);
+        D.status = c.take<PlanStatus>(1); D.tmp = c.take<uint8_t>(D.tmp_bytes);
+    };
+    Carve probe{nullptr};
+    lay(probe);
+    LURK_TRY(ensure(ctx->plan, probe.used));
+    Carve c{ctx->plan.as<uint8_t>()};
+    lay(c);
+    return LURK_OK;
+}
+
+// the device planner: n operations in device memory -> D and m, or the refusal plan_batch would give (LURK_ERR_ARG,
+// naming the same operation).  One read of the status word, after the ranks; the inserts are ordered only once the
+// batch is known to be accepted.
+template <class F>
+int plan_dev(lurk_trie_ctx *ctx, int n, const int32_t *kinds, const int64_t *prev, const F *roots, const F *keys, const F *values,
+             int fmt, cudaStream_t st, DevPlan<F> &D, int &m) {
+    const int H = ctx->height;
+    LURK_TRY(take_plan<F>(ctx, n, true, st, D));
+    LURK_CUDA_TRY(cudaMemsetAsync(D.status, 0xff, sizeof(PlanStatus), st));
+    LURK_CUDA_TRY(cudaMemsetAsync(D.first, 0xff, (size_t)n * 4, st));
+    first_continuer_kernel<<<blocks(n), TS_THREADS, 0, st>>>(n, kinds, prev, D.first);
+    validate_kernel<F><<<blocks(n), TS_THREADS, 0, st>>>(n, H, kinds, prev, roots, keys, values, fmt, D.first, D.ops, D.base, D.keys, D.vals,
+                                                         D.link_a, D.flags, D.status);
+    LURK_CUDA_TRY(cudaGetLastError());
+    uint32_t *head = D.link_a, *spare = D.link_b;
+    for (int r = 0; (1ll << r) < n; r++) {   // ceil(log2 n) rounds: every chain is shorter than n
+        jump_kernel<<<blocks(n), TS_THREADS, 0, st>>>(n, head, spare);
+        std::swap(head, spare);
+    }
+    size_t tb = D.tmp_bytes;
+    LURK_CUDA_TRY(cub::DeviceScan::InclusiveSum(D.tmp, tb, D.flags, D.incl, n, st));
+    const uint64_t fits = (ctx->capacity - ctx->count) / (uint64_t)H;
+    chain_rank_kernel<F><<<blocks(n), TS_THREADS, 0, st>>>(n, head, D.incl, fits, D.ops, D.base, D.order, D.status);
+    LURK_CUDA_TRY(cudaGetLastError());
+    PlanStatus s;
+    LURK_CUDA_TRY(cudaMemcpyAsync(&s, D.status, sizeof s, cudaMemcpyDeviceToHost, st));
+    LURK_CUDA_TRY(cudaStreamSynchronize(st));
+    if (s.err != NO_ERR) {
+        const size_t i = (size_t)(s.err >> 8);
+        int32_t k = 0;
+        int64_t j = 0;
+        LURK_CUDA_TRY(cudaMemcpy(&k, kinds + i, 4, cudaMemcpyDeviceToHost));
+        LURK_CUDA_TRY(cudaMemcpy(&j, prev + i, 8, cudaMemcpyDeviceToHost));
+        switch ((unsigned)(s.err & 0xff)) {
+        case PE_KIND: set_error("trie operation %zu: kind %d is neither LURK_TRIE_LOOKUP nor LURK_TRIE_INSERT", i, k); break;
+        case PE_PREV: set_error("trie operation %zu: prev %lld is not -1 or an earlier operation", i, (long long)j); break;
+        case PE_PREV_LOOKUP: set_error("trie operation %zu: prev %lld is a lookup, not an insert", i, (long long)j); break;
+        case PE_FORK: {
+            uint32_t f = 0;
+            LURK_CUDA_TRY(cudaMemcpy(&f, D.first + j, 4, cudaMemcpyDeviceToHost));
+            set_error("trie operation %zu: insert after insert %lld, which insert %u already continued (a fork inside a batch)", i, (long long)j, f);
+            break;
+        }
+        case PE_ROOTS_NULL: set_error("trie operation %zu: prev -1 names roots[%zu], but roots is NULL", i, i); break;
+        case PE_VALUES_NULL: set_error("trie operation %zu: an insert reads values[%zu], but values is NULL", i, i); break;
+        default: {
+            const unsigned c = (unsigned)(s.err & 0xff);
+            set_error("trie operation %zu: an element (%s) is not reduced below the field modulus", i, c == PE_ROOT ? "root" : (c == PE_KEY ? "key" : "value"));
+        }
+        }
+        return LURK_ERR_ARG;
+    }
+    m = (int)s.inserts;
+    if ((uint64_t)m * H > ctx->capacity - ctx->count) {
+        set_error("trie operation %u: insert %llu of the batch may add nodes past the capacity: %d inserts may add %llu nodes to a "
+                  "store of %llu nodes and capacity %llu", s.cap_first, (unsigned long long)fits, m, (unsigned long long)m * H,
+                  (unsigned long long)ctx->count, (unsigned long long)ctx->capacity);
+        return LURK_ERR_ARG;
+    }
+    if (m > 1) {
+        // stable least-significant-first passes: path word 0 .. the key's top word, then the chain -> (chain, path, index)
+        const int bits = 3 * H, chain_bits = 32 - __builtin_clz((unsigned)(n - 1));
+        cub::DoubleBuffer<uint32_t> key(D.key_a, D.key_b), ord(D.order, D.order_b);
+        for (int w = 0; w <= 8; w++) {
+            if (w < 8 && 32 * w >= bits) continue;
+            order_key_kernel<<<blocks(m), TS_THREADS, 0, st>>>(m, D.ops, ord.Current(), w, key.Current());
+            tb = D.tmp_bytes;
+            LURK_CUDA_TRY(cub::DeviceRadixSort::SortPairs(D.tmp, tb, key, ord, m, 0, w < 8 ? std::min(32, bits - 32 * w) : chain_bits, st));
+        }
+        D.order = ord.Current();
+    }
+    if (m) lcp_kernel<<<blocks(m), TS_THREADS, 0, st>>>(m, H, D.ops, D.order, D.lcp);
+    LURK_CUDA_TRY(cudaGetLastError());
+    return LURK_OK;
+}
+
+// the levels of one planned batch (steps 1-3 above), shared by both forms.  Results go to d_results (device, n elements
+// in fmt) when it is given, else to results_out (host, may be NULL).
+template <class F>
+int run_levels(lurk_trie_ctx *ctx, int n, int m, const DevPlan<F> &D, F *d_results, uint8_t *results_out, void *d_lookup, void *d_insert,
+               int fmt, cudaStream_t st) {
+    const int H = ctx->height;
+    const OpDev *ops = D.ops;
+    const F *base = D.base, *keys = D.keys, *vals = D.vals;
+    const uint32_t *order = D.order;
+    const int16_t *lcp = D.lcp;
     // CUB scratch for one scan and one sort of m keys
     size_t scan_bytes = 0, sort_bytes = 0;
     const int rank_bits = 33 - (m ? __builtin_clz((unsigned)m) : 32);
@@ -450,31 +705,21 @@ int apply_batch(lurk_trie_ctx *ctx, const Plan &P, uint8_t *results_out, void *d
         LURK_CUDA_TRY(cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, (const uint64_t *)nullptr, (uint64_t *)nullptr, m, 0, 32 + rank_bits, st));
     }
     Carve cv{nullptr};
-    auto lay = [&](Carve &c, OpDev *&ops, F *&base, F *&keys, F *&vals, F *&res, uint32_t *&nodes, uint32_t *&order, int16_t *&lcp,
-                   uint32_t *&flags, uint32_t *&rank, uint64_t *&kin, uint64_t *&kout, F *&dig_a, F *&dig_b, F *&newpre, uint32_t *&claim,
-                   void *&tmp) {
-        ops = c.take<OpDev>(n); base = c.take<F>(n); keys = c.take<F>(n); vals = c.take<F>(n); res = c.take<F>(n);
-        nodes = c.take<uint32_t>((size_t)n * H); order = c.take<uint32_t>(m); lcp = c.take<int16_t>(m); flags = c.take<uint32_t>(m);
-        rank = c.take<uint32_t>(m); kin = c.take<uint64_t>(m); kout = c.take<uint64_t>(m); dig_a = c.take<F>(m); dig_b = c.take<F>(m);
+    auto lay = [&](Carve &c, F *&res, uint32_t *&nodes, uint32_t *&flags, uint32_t *&rank, uint64_t *&kin, uint64_t *&kout, F *&dig_a,
+                   F *&dig_b, F *&newpre, uint32_t *&claim, void *&tmp) {
+        res = c.take<F>(n); nodes = c.take<uint32_t>((size_t)n * H); flags = c.take<uint32_t>(m); rank = c.take<uint32_t>(m);
+        kin = c.take<uint64_t>(m); kout = c.take<uint64_t>(m); dig_a = c.take<F>(m); dig_b = c.take<F>(m);
         newpre = c.take<F>((size_t)m * ARITY); claim = c.take<uint32_t>(m); tmp = c.take<uint8_t>(std::max(scan_bytes, sort_bytes));
     };
-    OpDev *ops; F *base, *keys, *vals, *res, *dig_a, *dig_b, *newpre; uint32_t *nodes, *order, *flags, *rank, *claim; int16_t *lcp;
+    F *res, *dig_a, *dig_b, *newpre; uint32_t *nodes, *flags, *rank, *claim;
     uint64_t *kin, *kout; void *tmp;
-    lay(cv, ops, base, keys, vals, res, nodes, order, lcp, flags, rank, kin, kout, dig_a, dig_b, newpre, claim, tmp);
-    LURK_TRY(ensure_scratch(ctx, cv.used));
+    lay(cv, res, nodes, flags, rank, kin, kout, dig_a, dig_b, newpre, claim, tmp);
+    LURK_TRY(ensure(ctx->scratch, cv.used));
     Carve c{ctx->scratch.as<uint8_t>()};
-    lay(c, ops, base, keys, vals, res, nodes, order, lcp, flags, rank, kin, kout, dig_a, dig_b, newpre, claim, tmp);
+    lay(c, res, nodes, flags, rank, kin, kout, dig_a, dig_b, newpre, claim, tmp);
+    if (d_results) res = d_results;   // written only once the walk found every node
     const size_t tmp_bytes = std::max(scan_bytes, sort_bytes);
     auto *err = ctx->err.as<unsigned long long>();
-
-    LURK_CUDA_TRY(cudaMemcpyAsync(ops, P.ops.data(), (size_t)n * sizeof(OpDev), cudaMemcpyHostToDevice, st));
-    LURK_CUDA_TRY(cudaMemcpyAsync(base, P.base.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
-    LURK_CUDA_TRY(cudaMemcpyAsync(keys, P.keys.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
-    LURK_CUDA_TRY(cudaMemcpyAsync(vals, P.vals.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
-    if (m) {
-        LURK_CUDA_TRY(cudaMemcpyAsync(order, P.order.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
-        LURK_CUDA_TRY(cudaMemcpyAsync(lcp, P.lcp.data(), (size_t)m * 2, cudaMemcpyHostToDevice, st));
-    }
     LURK_CUDA_TRY(cudaMemsetAsync(err, 0xff, 8, st));
 
     walk_kernel<F><<<blocks(n), TS_THREADS, 0, st>>>(n, H, ops, base, ctx->table.as<uint32_t>(), ctx->mask, ctx->dig.as<F>(), ctx->pre.as<F>(),
@@ -504,11 +749,13 @@ int apply_batch(lurk_trie_ctx *ctx, const Plan &P, uint8_t *results_out, void *d
         // the first operation whose walk missed a digest: its base root, or the child its parent node selects
         const int i = (int)(e >> 8), depth = (int)(e & 0xff);
         uint8_t miss[32];
-        if (depth == 0) memcpy(miss, &P.base[(size_t)i * 32], 32);
+        if (depth == 0) LURK_CUDA_TRY(cudaMemcpy(miss, base + i, 32, cudaMemcpyDeviceToHost));
         else {
             uint32_t parent = 0;
+            OpDev o;
             LURK_CUDA_TRY(cudaMemcpy(&parent, nodes + (size_t)(depth - 1) * n + i, 4, cudaMemcpyDeviceToHost));
-            LURK_CUDA_TRY(cudaMemcpy(miss, ctx->pre.as<F>() + (size_t)parent * ARITY + chunk_at(P.ops[i].path, H, depth - 1), 32,
+            LURK_CUDA_TRY(cudaMemcpy(&o, ops + i, sizeof o, cudaMemcpyDeviceToHost));
+            LURK_CUDA_TRY(cudaMemcpy(miss, ctx->pre.as<F>() + (size_t)parent * ARITY + chunk_at(o.path, H, depth - 1), 32,
                                      cudaMemcpyDeviceToHost));
         }
         char hex[65];
@@ -518,6 +765,23 @@ int apply_batch(lurk_trie_ctx *ctx, const Plan &P, uint8_t *results_out, void *d
     }
     if (results_out) LURK_CUDA_TRY(cudaMemcpy(results_out, res, (size_t)n * 32, cudaMemcpyDeviceToHost));
     return LURK_OK;
+}
+
+// the host form: upload plan_batch's plan, then the levels
+template <class F>
+int apply_batch(lurk_trie_ctx *ctx, const Plan &P, uint8_t *results_out, void *d_lookup, void *d_insert, int fmt, cudaStream_t st) {
+    const int n = (int)P.ops.size(), m = P.inserts;
+    DevPlan<F> D;
+    LURK_TRY(take_plan<F>(ctx, n, false, st, D));
+    LURK_CUDA_TRY(cudaMemcpyAsync(D.ops, P.ops.data(), (size_t)n * sizeof(OpDev), cudaMemcpyHostToDevice, st));
+    LURK_CUDA_TRY(cudaMemcpyAsync(D.base, P.base.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
+    LURK_CUDA_TRY(cudaMemcpyAsync(D.keys, P.keys.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
+    LURK_CUDA_TRY(cudaMemcpyAsync(D.vals, P.vals.data(), (size_t)n * 32, cudaMemcpyHostToDevice, st));
+    if (m) {
+        LURK_CUDA_TRY(cudaMemcpyAsync(D.order, P.order.data(), (size_t)m * 4, cudaMemcpyHostToDevice, st));
+        LURK_CUDA_TRY(cudaMemcpyAsync(D.lcp, P.lcp.data(), (size_t)m * 2, cudaMemcpyHostToDevice, st));
+    }
+    return run_levels<F>(ctx, n, m, D, nullptr, results_out, d_lookup, d_insert, fmt, st);
 }
 
 int ctx_ready(lurk_trie_ctx *ctx) {
@@ -628,6 +892,67 @@ int lurk_trie_ctx_apply(lurk_trie_ctx *ctx, size_t n, const int *kinds, const in
         LURK_TRY(ctx_ready(ctx));
         if (!n) return LURK_OK;
         return apply_batch<F>(ctx, P, results_out, d_lookup_inputs, d_insert_inputs, fmt, (cudaStream_t)stream);
+    });
+}
+
+int lurk_trie_ctx_register_dev(lurk_trie_ctx *ctx, const void *d_preimages, size_t n, void *d_digests_out, int fmt, void *stream) {
+    if (!ctx) { set_error("null trie context"); return LURK_ERR_ARG; }
+    if (fmt != LURK_FMT_CANONICAL && fmt != LURK_FMT_MONTGOMERY) { set_error("bad format %d", fmt); return LURK_ERR_ARG; }
+    if (n && !d_preimages) { set_error("null preimages"); return LURK_ERR_ARG; }
+    if (n > ctx->capacity - ctx->count) {
+        set_error("trie register: %zu nodes into a store of %llu nodes and capacity %llu", n, (unsigned long long)ctx->count,
+                  (unsigned long long)ctx->capacity);
+        return LURK_ERR_ARG;
+    }
+    return dispatch_field(ctx->field_id, [&](auto f) {
+        using F = decltype(f);
+        LURK_TRY(ctx_ready(ctx));
+        if (!n) return LURK_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        F *pre, *dig;
+        uint32_t *claim;
+        unsigned long long *bad;
+        auto lay = [&](Carve &c) { pre = c.take<F>(n * ARITY); dig = c.take<F>(n); claim = c.take<uint32_t>(n); bad = c.take<unsigned long long>(1); };
+        Carve probe{nullptr};
+        lay(probe);
+        LURK_TRY(ensure(ctx->plan, probe.used));
+        Carve c{ctx->plan.as<uint8_t>()};
+        lay(c);
+        LURK_CUDA_TRY(cudaMemsetAsync(bad, 0xff, 8, st));
+        canon_check_kernel<F><<<blocks(n * ARITY), TS_THREADS, 0, st>>>(n * ARITY, (const F *)d_preimages, fmt, pre, bad);
+        LURK_CUDA_TRY(cudaGetLastError());
+        unsigned long long e = NO_ERR;
+        LURK_CUDA_TRY(cudaMemcpyAsync(&e, bad, 8, cudaMemcpyDeviceToHost, st));
+        LURK_CUDA_TRY(cudaStreamSynchronize(st));
+        if (e != NO_ERR) {
+            set_error("trie register: preimage %llu element %llu is not reduced below the field modulus", e / ARITY, e % ARITY);
+            return LURK_ERR_ARG;
+        }
+        LURK_CUDA_TRY(cudaMemsetAsync(ctx->err.p, 0xff, 8, st));
+        LURK_TRY(register_dev<F>(ctx, pre, dig, claim, (int)n, st));
+        if (d_digests_out) {
+            if (fmt == LURK_FMT_MONTGOMERY) LURK_TRY(convert_dev<F>(dig, n, LURK_FMT_MONTGOMERY, d_digests_out, st));
+            else LURK_CUDA_TRY(cudaMemcpyAsync(d_digests_out, dig, n * 32, cudaMemcpyDeviceToDevice, st));
+        }
+        return sync_count(ctx, st);
+    });
+}
+
+int lurk_trie_ctx_apply_dev(lurk_trie_ctx *ctx, size_t n, const int32_t *d_kinds, const int64_t *d_prev, const void *d_roots, const void *d_keys,
+                            const void *d_values, int fmt, void *d_results, void *d_lookup_inputs, void *d_insert_inputs, void *stream) {
+    if (!ctx) { set_error("null trie context"); return LURK_ERR_ARG; }
+    if (fmt != LURK_FMT_CANONICAL && fmt != LURK_FMT_MONTGOMERY) { set_error("bad format %d", fmt); return LURK_ERR_ARG; }
+    if (n && (!d_kinds || !d_prev || !d_keys)) { set_error("null kinds, prev or keys"); return LURK_ERR_ARG; }
+    if (n >= (size_t)1 << 31) { set_error("trie batch of %zu operations: at most 2^31 - 1", n); return LURK_ERR_ARG; }
+    return dispatch_field(ctx->field_id, [&](auto f) {
+        using F = decltype(f);
+        LURK_TRY(ctx_ready(ctx));
+        if (!n) return LURK_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        DevPlan<F> D;
+        int m = 0;
+        LURK_TRY(plan_dev<F>(ctx, (int)n, d_kinds, d_prev, (const F *)d_roots, (const F *)d_keys, (const F *)d_values, fmt, st, D, m));
+        return run_levels<F>(ctx, (int)n, m, D, (F *)d_results, nullptr, d_lookup_inputs, d_insert_inputs, fmt, st);
     });
 }
 

@@ -163,6 +163,13 @@ class DeviceTrie:
     def __init__(self, field_id=_capi.FIELD_BN254_FR, height=85, capacity=1 << 20):
         self.field_id, self.height = field_id, height
         self._lib = _capi.lib()
+        # the store is built on the CUDA device current at creation (torch's, once torch has made its context current):
+        # the _dev calls take tensors on that device only
+        self._device = None
+        if self._lib.lurk_device_count() > 0:
+            import torch
+            if torch.cuda.is_available():
+                self._device = torch.cuda.current_device()
         ctx = C.c_void_p()
         _capi.check(self._lib.lurk_trie_ctx_create(field_id, height, capacity, C.byref(ctx)))
         self._ctx = ctx
@@ -233,6 +240,109 @@ class DeviceTrie:
                                                   _capi.np_ptr(vals), fmt, _capi.np_ptr(res), lookup_out.data_ptr() if lookup_out.numel() else None,
                                                   insert_out.data_ptr() if insert_out.numel() else None, stream))
         return unpack(res), lookup_out, insert_out
+
+    def register_dev(self, preimages, fmt=_capi.FMT_CANONICAL, digests_out=None, stream=None):
+        """`register` on device memory: preimages a contiguous uint8 CUDA tensor of (n, 8, 32), elements in fmt.
+        Returns the digests as a uint8 CUDA tensor of (n, 32) in fmt (digests_out when given)."""
+        import torch
+        _check_dev("preimages", preimages, torch.uint8, 3)
+        n = preimages.shape[0]
+        if tuple(preimages.shape[1:]) != (8, 32):
+            raise ValueError(f"preimages must be (n, 8, 32), not {tuple(preimages.shape)}")
+        if digests_out is not None:
+            _check_dev("digests_out", digests_out, torch.uint8, 2, (n, 32))
+        self._on_store_device(preimages=preimages, digests_out=digests_out)
+        st = _call_stream(torch, stream, preimages.device)
+        with torch.cuda.stream(st):
+            if digests_out is None:
+                digests_out = torch.empty((n, 32), dtype=torch.uint8, device=preimages.device)
+        _capi.check(self._lib.lurk_trie_ctx_register_dev(self._ctx, _dptr(preimages), n, _dptr(digests_out), fmt, st.cuda_stream))
+        return digests_out
+
+    def apply_dev(self, kinds, prev, roots, keys, values, fmt=_capi.FMT_CANONICAL, results=None, lookup_out=None, insert_out=None, stream=None):
+        """`apply` on operations already in device memory, planned on the GPU: kinds int32 (n,), prev int64 (n,), roots /
+        keys / values uint8 (n, 32) in fmt, all contiguous CUDA tensors; roots or values may be None when never read.
+        Returns (results, lookup_inputs, insert_inputs) as uint8 CUDA tensors of (n, 32), (lookups, 2 + 8H, 32) and
+        (inserts, 3 + 16H, 32), in fmt; results / lookup_out / insert_out: caller tensors to write into instead, of exactly
+        the batch's size.  stream: the CUDA stream handle the call is ordered on (default: torch's current stream); the
+        batch's insert count, which sizes the proof buffers, is read on that stream too, after the caller's work there."""
+        import torch
+        _check_dev("kinds", kinds, torch.int32, 1)
+        n = kinds.shape[0]
+        _check_dev("prev", prev, torch.int64, 1, (n,))
+        _check_dev("keys", keys, torch.uint8, 2, (n, 32))
+        for name, t in (("roots", roots), ("values", values)):
+            if t is not None:
+                _check_dev(name, t, torch.uint8, 2, (n, 32))
+        for name, t in (("results", results), ("lookup_out", lookup_out), ("insert_out", insert_out)):
+            if t is not None:
+                _check_dev(name, t, torch.uint8, 2 if name == "results" else None, (n, 32) if name == "results" else None)
+        self._on_store_device(kinds=kinds, prev=prev, roots=roots, keys=keys, values=values, results=results, lookup_out=lookup_out,
+                              insert_out=insert_out)
+        H, dev = self.height, kinds.device
+        st = _call_stream(torch, stream, dev)
+        with torch.cuda.stream(st):
+            # the proofs are written at rank x proof size: every buffer must hold exactly the batch's lookups or inserts
+            n_ins = int((kinds == TRIE_INSERT).sum())
+            if results is None:
+                results = torch.empty((n, 32), dtype=torch.uint8, device=dev)
+            if lookup_out is None:
+                lookup_out = torch.empty((n - n_ins, trie_n_inputs(TRIE_LOOKUP, H), 32), dtype=torch.uint8, device=dev)
+            if insert_out is None:
+                insert_out = torch.empty((n_ins, trie_n_inputs(TRIE_INSERT, H), 32), dtype=torch.uint8, device=dev)
+        for name, out, op, count in (("lookup_out", lookup_out, TRIE_LOOKUP, n - n_ins), ("insert_out", insert_out, TRIE_INSERT, n_ins)):
+            want = count * trie_n_inputs(op, H) * 32
+            if out.numel() != want:
+                raise ValueError(f"{name} must hold the batch's {count} proofs of {trie_n_inputs(op, H)} elements ({want} bytes), "
+                                 f"not {out.numel()} bytes")
+        _capi.check(self._lib.lurk_trie_ctx_apply_dev(self._ctx, n, _dptr(kinds), _dptr(prev), _dptr(roots), _dptr(keys), _dptr(values), fmt,
+                                                      _dptr(results), _dptr(lookup_out), _dptr(insert_out), st.cuda_stream))
+        return results, lookup_out, insert_out
+
+    def _on_store_device(self, **tensors):
+        """every tensor given is on a CUDA device, the one the store was built on, else ValueError"""
+        _on_cuda(**tensors)
+        for name, t in tensors.items():
+            if t is not None and self._device is not None and t.device.index != self._device:
+                raise ValueError(f"{name} is on {t.device}, but the trie store was built on cuda:{self._device}")
+
+
+def _call_stream(torch, stream, device):
+    """the torch stream of a call: torch's current one on the device, or the caller's handle"""
+    current = torch.cuda.current_stream(device)
+    if stream is None or int(stream) == current.cuda_stream:
+        return current
+    return torch.cuda.ExternalStream(int(stream), device=device)
+
+
+def _dptr(t):
+    return t.data_ptr() if t is not None and t.numel() else None
+
+
+def _check_dev(name, t, dtype, ndim, shape=None):
+    """a contiguous tensor of this dtype (and rank and shape when given), else ValueError; _on_cuda checks the device"""
+    import torch
+    if not isinstance(t, torch.Tensor):
+        raise ValueError(f"{name} must be a CUDA tensor, not {type(t).__name__}")
+    if t.dtype != dtype:
+        raise ValueError(f"{name} must be {dtype}, not {t.dtype}")
+    if (ndim is not None and t.dim() != ndim) or (shape is not None and tuple(t.shape) != tuple(shape)):
+        raise ValueError(f"{name} has shape {tuple(t.shape)}, not {tuple(shape) if shape is not None else f'{ndim} dimensions'}")
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+
+
+def _on_cuda(**tensors):
+    """every tensor given (None: not given) is on one CUDA device, else ValueError"""
+    devices = set()
+    for name, t in tensors.items():
+        if t is None:
+            continue
+        if not t.is_cuda:
+            raise ValueError(f"{name} must be on a CUDA device, not {t.device}")
+        devices.add(t.device)
+    if len(devices) > 1:
+        raise ValueError(f"the tensors are on more than one device: {sorted(str(d) for d in devices)}")
 
 
 def write_trie_batch(device_trie, fold_ctx, b, batch_index, ops):
