@@ -199,8 +199,7 @@ struct FoldCtx final : FoldCtxBase {
         {
             // commit(W2 - D): after the dummy-witness offset only ~a third of the scalars are non-zero, so the 2^(c-1)-bucket
             // reduction weighs more against the per-window additions than for a dense vector: own narrower table when it pays
-            static const int w_window_env = [] { const char *e = getenv("LURK_FOLD_W_WINDOW"); return e ? atoi(e) : 0; }();   // tuning aid
-            const int want = std::min(ck_w->fixed_c, w_window_env ? w_window_env : FOLD_W_WINDOW);
+            const int want = std::min(ck_w->fixed_c, FOLD_W_WINDOW);
             LURK_TRY(lurk_msm_ctx_clone(ck_w, &ckWbase));
             if (want != ck_w->fixed_c && c.n_w) {
                 ckWbase->n = c.n_w;
@@ -216,8 +215,7 @@ struct FoldCtx final : FoldCtxBase {
             // commit(T) sits on the sequential chain: a narrower window than the throughput optimum shortens the bucket
             // reduction (2^(c-1) buckets on the critical path) at the price of a few more additions per scalar; the context
             // gets its own table over exactly n_rows bases
-            static const int t_window_env = [] { const char *e = getenv("LURK_FOLD_T_WINDOW"); return e ? atoi(e) : 0; }();   // tuning aid
-            const int want = std::min(ck_t->fixed_c, t_window_env ? t_window_env : FOLD_T_WINDOW);   // never wider than the key's own choice
+            const int want = std::min(ck_t->fixed_c, FOLD_T_WINDOW);   // never wider than the key's own choice
             if (want != ck_t->fixed_c && c.n_rows) {
                 ckT->n = c.n_rows;
                 ckT->d_table = nullptr;
@@ -563,10 +561,9 @@ struct FoldCtx final : FoldCtxBase {
     int prepare_dummy() {
         if (dummy_ready) return LURK_OK;
         dummy_ready = true;
-        static const bool off = getenv("LURK_FOLD_NO_DUMMY_OFFSET") != nullptr;      // measurement aid
         size_t nslots = 0;
         for (auto &sb : batches) nslots += sb->coprocessor() ? 0 : sb->count;   // coprocessor blocks are not part of D
-        if (off || !nslots || !cfg.n_w) return LURK_OK;
+        if (!nslots || !cfg.n_w) return LURK_OK;
         LURK_TRY(dummy_w.alloc((size_t)cfg.n_w * sizeof(Fs)));
         LURK_CUDA_TRY(cudaMemsetAsync(dummy_w.p, 0, (size_t)cfg.n_w * sizeof(Fs), sB));
         for (auto &sb : batches) {
@@ -604,9 +601,6 @@ struct FoldCtx final : FoldCtxBase {
         if (fmt != LURK_FMT_CANONICAL && fmt != LURK_FMT_MONTGOMERY) { set_error("bad format %d", fmt); return LURK_ERR_ARG; }
         if (b_pending[b]) { set_error("buffer %d: the previous step's result has not been collected", b); return LURK_ERR_ARG; }
         const bool staged = !(flags & FOLD_INPUTS_RESIDENT);
-        // measurement aid: with resident inputs, re-use the fresh instance already prepared in this buffer (the chain alone)
-        static const bool skip_a = getenv("LURK_FOLD_SKIP_STAGE_A") != nullptr;
-        if (skip_a && !staged && a_recorded[b]) return LURK_OK;
         if (!staged && fmt != LURK_FMT_MONTGOMERY) { set_error("device-resident inputs are Montgomery form"); return LURK_ERR_ARG; }
         Fs *W2 = z2[b].as<Fs>();
         unsigned k = 0;

@@ -52,6 +52,7 @@ struct MsmPlan {
     uint32_t rwin = 0, K = 0, G = 0, nq = 0, SL = 0, slice = 0;
 };
 static constexpr uint32_t MSM_MAX_RESULT_POINTS = 512;    // rwin * nq <= 64 * 1 .. 13 * 17: read back per commitment
+static constexpr uint32_t MSM_MAX_SEG = 32;                // longest segment of the sorted list one level-1 thread accumulates
 
 // Window width of the fixed-base mode: 2^(c-1) buckets for ~n * 254 / c entries.  c = 20 from half a million bases up (the
 // step circuit's witness, 911 900 terms, and a 2^21-point key get the same 13 windows); smaller keys keep >= 20 entries per
@@ -81,8 +82,7 @@ inline MsmPlan make_plan(size_t n, int scalar_bits, int fixed_c = 0) {
     size_t cap = n * (size_t)p.nwin;
     size_t want_threads = (size_t)sm_count() * 1024;
     size_t seg = (cap + want_threads - 1) / want_threads;
-    static const size_t seg_cap = [] { const char *e = getenv("LURK_MSM_SEG"); return e ? (size_t)atoi(e) : (size_t)32; }();   // tuning aid
-    p.seg = (uint32_t)std::min<size_t>(seg_cap, std::max<size_t>(8, seg));
+    p.seg = (uint32_t)std::min<size_t>(MSM_MAX_SEG, std::max<size_t>(8, seg));
     p.t1 = (uint32_t)((cap + p.seg - 1) / p.seg);
     if (p.t1 == 0) p.t1 = 1;
     return p;
@@ -182,11 +182,10 @@ __host__ __device__ __forceinline__ BucketPartials bucket_partials(uint32_t lo, 
 // buckets with more partials than this are merged by a whole CTA (msm_merge_long_kernel); the others by one thread each
 static constexpr uint32_t MSM_LONG_PARTIALS = 16;
 
-// long_list (optional): appends every bucket with more than MSM_LONG_PARTIALS partials for segments of `seg` entries;
-// long_list[-1] is its length, zeroed before the launch
+// long_list: appends every bucket with more than MSM_LONG_PARTIALS partials for segments of `seg` entries; long_list[-1] is its
+// length, zeroed before the launch
 static __global__ void __launch_bounds__(1024) msm_scan_apply_kernel(const uint32_t *__restrict__ counts, uint32_t len, const uint32_t *__restrict__ tile_offsets,
-                                                              uint32_t ntiles, uint32_t *__restrict__ offsets, uint32_t seg = 0,
-                                                              uint32_t *long_list = nullptr) {
+                                                              uint32_t ntiles, uint32_t *__restrict__ offsets, uint32_t seg, uint32_t *long_list) {
     const uint32_t base = blockIdx.x * SCAN_TILE + threadIdx.x * 4;
     uint32_t v[4], sum = 0;
 #pragma unroll
@@ -196,7 +195,7 @@ static __global__ void __launch_bounds__(1024) msm_scan_apply_kernel(const uint3
     for (int k = 0; k < 4; k++) {
         if (base + k < len) {
             offsets[base + k] = run;
-            if (long_list && bucket_partials(run, run + v[k], seg).count > MSM_LONG_PARTIALS) long_list[atomicAdd(long_list - 1, 1u)] = base + k;
+            if (bucket_partials(run, run + v[k], seg).count > MSM_LONG_PARTIALS) long_list[atomicAdd(long_list - 1, 1u)] = base + k;
         }
         run += v[k];
     }
@@ -517,8 +516,7 @@ __device__ __forceinline__ void store_xyzz(XYZZ<Fb> *p, const XYZZ<Fb> &a) {
 // level 1: fixed-length segments of the sorted list
 // MINB = resident CTAs per SM the register allocation is held to: 4 (126 registers, no spills) is best while the key is
 // L2 resident; the fixed-base table (1.7 GB, DRAM gathers) gains ~5 % from 5 CTAs (96 registers, ~150 B of spills).
-// DIRECT: the list is already a list of affine points (the output of the pair rounds below): entry `pos` is bases[pos], no sign
-template <class Fb, int MINB, bool DIRECT = false>
+template <class Fb, int MINB>
 __global__ void __launch_bounds__(128, MINB) msm_accumulate_kernel(const uint32_t *__restrict__ offsets, uint32_t nbuckets,
                                                              const uint32_t *__restrict__ sorted, const Affine<Fb> *__restrict__ bases,
                                                              XYZZ<Fb> *__restrict__ bucket_acc, XYZZ<Fb> *__restrict__ ppt, uint32_t seg,
@@ -541,7 +539,7 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate_kernel(const uint32_
     // a first run that starts inside its bucket continues another thread's run: it becomes the partial ppt[t], which
     // msm_merge_kernel adds to the bucket (see bucket_partials); every other run starts its bucket and writes it
     bool first_run = offsets[key] != start;
-    uint32_t e_next = DIRECT ? start : sorted[start];
+    uint32_t e_next = sorted[start];
     Affine<Fb> p_next = load_affine(bases + (e_next & 0x7fffffffu));
     XYZZ<Fb> acc = XYZZ<Fb>::identity();
     // ONE flat loop over the segment: every lane performs exactly one addition per iteration, so lanes whose bucket
@@ -552,7 +550,7 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate_kernel(const uint32_
         const Affine<Fb> p = p_next;
         pos++;
         if (pos < end) {   // prefetch the next entry while this addition runs
-            e_next = DIRECT ? pos : sorted[pos];
+            e_next = sorted[pos];
             p_next = load_affine(bases + (e_next & 0x7fffffffu));
         }
         acc.add_affine(p, (e >> 31) != 0);
@@ -566,141 +564,6 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate_kernel(const uint32_
                 run_end = min(offsets[key + 1], end);
             }
         }
-    }
-}
-
-// ---- pair rounds: batched-affine additions in front of the XYZZ accumulation ------------------------------------------------
-// A mixed XYZZ addition costs 10 field products; an AFFINE addition costs 3 (lambda = dy / dx; x3 = lambda^2 - x1 - x2;
-// y3 = lambda (x1 - x3) - y1) plus one inversion -- and inversions batch: Montgomery's trick turns the inversions of a whole CTA
-// warp (32 threads x PAIR_B additions) into ONE inversion (binary GCD, on the ALU pipe, by one lane) + 3 products per addition + a
-// dozen products per thread for the cross-lane prefix / suffix products.  ~7 products per addition instead of 10.
-// Independent additions come from the sorted list itself: inside every bucket's run, entries 2j and 2j + 1 are added pairwise (an odd
-// tail is copied), which halves every run: out run k has ceil(m_k / 2) affine points.  One or two such rounds (half resp. three
-// quarters of all additions) run before the fixed-length-segment XYZZ accumulation takes the rest.
-static constexpr int PAIR_B = 16;        // output points per thread and batch
-// default number of pair rounds for long / short average runs: 0 = off (one round makes the fold step slower as implemented,
-// 4.94 vs 4.34 ms on an H100 at 400 W: the per-batch inversion stalls its CTA) -- LURK_MSM_PAIR_ROUNDS overrides
-static constexpr int MSM_PAIR_ROUNDS_LONG = 0, MSM_PAIR_ROUNDS_SHORT = 0;
-
-static __global__ void __launch_bounds__(256) msm_halve_kernel(const uint32_t *__restrict__ offs_in, uint32_t nbuckets, uint32_t *__restrict__ counts_out) {
-    for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k <= nbuckets; k += gridDim.x * blockDim.x)
-        counts_out[k] = k < nbuckets ? (offs_in[k + 1] - offs_in[k] + 1u) >> 1 : 0u;
-}
-
-// the two inputs of output slot q of bucket k and how they combine
-template <class Fb>
-struct PairIn {
-    Affine<Fb> p1, p2;
-    int kind;            // 0 copy p1, 1 chord addition, 2 doubling of p1, 3 result is the identity
-};
-template <class Fb, bool FIRST>
-__device__ __forceinline__ Affine<Fb> pair_load(const uint32_t *__restrict__ sorted, const Affine<Fb> *__restrict__ pts, uint32_t pos) {
-    if (!FIRST) return load_affine(pts + pos);
-    const uint32_t e = sorted[pos];
-    Affine<Fb> p = load_affine(pts + (e & 0x7fffffffu));
-    if (e >> 31) p.y = p.y.neg();
-    return p;
-}
-template <class Fb, bool FIRST>
-__device__ __forceinline__ PairIn<Fb> pair_fetch(const uint32_t *__restrict__ sorted, const Affine<Fb> *__restrict__ pts, uint32_t in, uint32_t run_end) {
-    PairIn<Fb> r;
-    r.p1 = pair_load<Fb, FIRST>(sorted, pts, in);
-    r.kind = 0;
-    r.p2 = r.p1;
-    if (in + 1 < run_end) {
-        r.p2 = pair_load<Fb, FIRST>(sorted, pts, in + 1);
-        if (r.p1.is_identity()) { r.p1 = r.p2; }                       // 0 + Q: copy Q
-        else if (r.p2.is_identity()) {}                                  // P + 0: copy P
-        else if (r.p1.x == r.p2.x) r.kind = (r.p1.y == r.p2.y && !r.p1.y.is_zero()) ? 2 : 3;
-        else r.kind = 1;
-    }
-    return r;
-}
-template <class Fb>
-__device__ __forceinline__ Fb pair_denominator(const PairIn<Fb> &in) {
-    if (in.kind == 1) return in.p2.x - in.p1.x;
-    if (in.kind == 2) return in.p1.y.dbl();
-    return Fb::one();
-}
-
-// 1 / v for every lane of a warp with ONE field inversion (v != 0 everywhere): inclusive prefix and suffix products by shuffles,
-// lane 31 inverts the total (binary GCD: shifts and adds on the ALU pipe, the multiplier stays free for the other warps of the SM)
-template <class Fb>
-__device__ __forceinline__ Fb warp_batch_inverse(const Fb &v) {
-    const int lane = threadIdx.x & 31;
-    Fb pre = v, suf = v;
-#pragma unroll 1
-    for (int d = 1; d < 32; d <<= 1) {
-        Fb a, b;
-#pragma unroll
-        for (int i = 0; i < 8; i++) { a.v[i] = __shfl_up_sync(0xffffffffu, pre.v[i], d); b.v[i] = __shfl_down_sync(0xffffffffu, suf.v[i], d); }
-        if (lane >= d) pre = pre * a;
-        if (lane + d < 32) suf = suf * b;
-    }
-    Fb inv = Fb::zero();
-    if (lane == 31) inv = pre.inv_vartime();
-    Fb ep, es, r;                                  // exclusive prefix / suffix, inverse of the warp total
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-        ep.v[i] = __shfl_up_sync(0xffffffffu, pre.v[i], 1);
-        es.v[i] = __shfl_down_sync(0xffffffffu, suf.v[i], 1);
-        r.v[i] = __shfl_sync(0xffffffffu, inv.v[i], 31);
-    }
-    if (lane > 0) r = r * ep;
-    if (lane < 31) r = r * es;
-    return r;
-}
-
-// One pair round.  offs_in / offs_out: bucket offsets of the input / output lists (offs_out = scan of ceil(m / 2)).
-// Thread t produces output slots [t * PAIR_B, (t + 1) * PAIR_B); a warp shares one inversion per batch of 32 x PAIR_B additions.
-template <class Fb, bool FIRST>
-__global__ void __launch_bounds__(128) msm_pair_kernel(const uint32_t *__restrict__ offs_in, const uint32_t *__restrict__ offs_out, uint32_t nbuckets,
-                                                       const uint32_t *__restrict__ sorted, const Affine<Fb> *__restrict__ pts_in,
-                                                       Affine<Fb> *__restrict__ pts_out) {
-    const uint32_t total = offs_out[nbuckets];
-    const uint64_t gtid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if ((gtid & ~31ull) * PAIR_B >= total) return;                              // the whole warp is past the end
-    const uint64_t start64 = gtid * PAIR_B;
-    const bool active = start64 < total;
-    const uint32_t start = active ? (uint32_t)start64 : 0, end = active ? (uint32_t)min((uint64_t)total, start64 + PAIR_B) : 0;
-    uint32_t k = 0;
-    if (active) {
-        uint32_t lo = 0, hi = nbuckets;
-        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (offs_out[mid] <= start) lo = mid; else hi = mid; }
-        k = lo;
-    }
-    Fb pref[PAIR_B];                                 // running products of the denominators (thread-private, L1-resident)
-    Fb run = Fb::one();
-    for (uint32_t q = start; q < end; q++) {
-        while (offs_out[k + 1] <= q) k++;
-        const uint32_t in = offs_in[k] + 2 * (q - offs_out[k]);
-        const PairIn<Fb> pi = pair_fetch<Fb, FIRST>(sorted, pts_in, in, offs_in[k + 1]);
-        run = run * pair_denominator(pi);
-        pref[q - start] = run;
-    }
-    Fb inv = warp_batch_inverse(run);              // 1 / (product of this thread's denominators)
-    // backwards: peel one denominator at a time
-    for (uint32_t q = end; q-- > start;) {
-        while (offs_out[k] > q) k--;
-        const uint32_t in = offs_in[k] + 2 * (q - offs_out[k]);
-        const PairIn<Fb> pi = pair_fetch<Fb, FIRST>(sorted, pts_in, in, offs_in[k + 1]);
-        const uint32_t j = q - start;
-        const Fb den = pair_denominator(pi);
-        const Fb inv_d = j ? inv * pref[j - 1] : inv;     // 1 / den
-        inv = inv * den;
-        Affine<Fb> o = pi.p1;
-        if (pi.kind == 3) { o.x = Fb::zero(); o.y = Fb::zero(); }
-        else if (pi.kind) {
-            Fb num;
-            if (pi.kind == 1) num = pi.p2.y - pi.p1.y;
-            else { const Fb xx = pi.p1.x.sqr(); num = xx.dbl() + xx; }
-            const Fb lam = num * inv_d;
-            const Fb x3 = lam.sqr() - pi.p1.x - pi.p2.x;
-            o.y = lam * (pi.p1.x - x3) - pi.p1.y;
-            o.x = x3;
-        }
-        store_fe(&pts_out[q].x, o.x);
-        store_fe(&pts_out[q].y, o.y);
     }
 }
 
@@ -924,7 +787,7 @@ __global__ void __launch_bounds__(256) msm_bases_to_mont_kernel(Fb *coords, size
 
 // ----------------------------------------------------------------------------- context
 struct MsmScratch {
-    DevBuf counts, hist, offsets, tiles, sorted, parts, buckets, ppt, chunks, chunk_sums, slices, wins, result, scalars, pair_offs[2], pair_pts[2];
+    DevBuf counts, hist, offsets, tiles, sorted, parts, buckets, ppt, chunks, chunk_sums, slices, wins, result, scalars;
     void *h_wins = nullptr;   // pinned
     void *h_stage[2] = {nullptr, nullptr};          // pinned staging for host-buffer scalars
     cudaEvent_t stage_done[2] = {nullptr, nullptr};
@@ -1026,22 +889,8 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     if ((uint64_t)n * (uint64_t)P.nwin >= (1ull << 32)) { set_error("%zu scalars exceed one launch (shard the commitment key)", n); return LURK_ERR_ARG; }
     const uint32_t TB = P.total_buckets;
     const uint32_t ntiles = (TB + SCAN_TILE - 1) / SCAN_TILE;
-    // pair rounds (batched-affine additions in front of the XYZZ accumulation): only when the runs are long enough to pair
-    const size_t cap = n * (size_t)P.nwin;
-    int rounds = 0;
-    {
-        static const int forced = [] { const char *e = getenv("LURK_MSM_PAIR_ROUNDS"); return e ? atoi(e) : -1; }();   // tuning aid
-        const size_t avg = cap / TB;
-        if (forced >= 0) rounds = forced;
-        else if (n >= 8192) rounds = avg >= 12 ? MSM_PAIR_ROUNDS_LONG : (avg >= 5 ? MSM_PAIR_ROUNDS_SHORT : 0);
-        if (rounds > 4) rounds = 4;
-    }
-    size_t cap_final = cap;
-    for (int r = 0; r < rounds; r++) cap_final = cap_final / 2 + TB + 1;       // sum of ceil(m_k / 2) <= cap / 2 + buckets
-    const uint32_t t1 = rounds ? (uint32_t)((cap_final + P.seg - 1) / P.seg) : P.t1;
-    const uint32_t t1_alloc = std::max(t1, P.t1);
     // a long bucket holds more than MSM_LONG_PARTIALS segment starts, so there are at most t1 / (MSM_LONG_PARTIALS + 1)
-    const uint32_t max_long = t1 / (MSM_LONG_PARTIALS + 1) + 1;
+    const uint32_t max_long = P.t1 / (MSM_LONG_PARTIALS + 1) + 1;
     // digit sort: per-CTA shared-memory histograms and two coalesced passes when one bucket set fits a CTA's shared memory (see
     // msm_hist_smem_kernel).
     // LURK_MSM_SORT=legacy forces the global-atomics kernels (tuning aid, read at every launch so that one process can compare both)
@@ -1060,7 +909,7 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
         LURK_TRY(ensure(S.tiles, ((size_t)ntiles + 1) * 2 * sizeof(uint32_t)));  // tile sums | tile offsets
         LURK_TRY(ensure(S.sorted, n * (size_t)P.nwin * sizeof(uint32_t)));
         LURK_TRY(ensure(S.buckets, (size_t)TB * sizeof(Pt)));
-        LURK_TRY(ensure(S.ppt, (size_t)t1_alloc * sizeof(Pt)));              // one partial slot per level-1 thread
+        LURK_TRY(ensure(S.ppt, (size_t)P.t1 * sizeof(Pt)));              // one partial slot per level-1 thread
         const size_t nchunks_all = (size_t)P.rwin * P.G;
         LURK_TRY(ensure(S.chunks, nchunks_all * sizeof(Pt)));          // tri_g
         LURK_TRY(ensure(S.chunk_sums, nchunks_all * sizeof(Pt)));      // run_g
@@ -1098,7 +947,7 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
         msm_hist_smem_kernel<Fs><<<sort_ctas, MSM_SORT_THREADS, smem, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, P.nb, cnt, rng, tile_sums, ntiles);
         msm_hist_columns_kernel<<<(P.nb + 255) / 256, 256, 0, s>>>(cnt, rng, sort_ctas, P.nb, counts, cursor, tile_sums);
         msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
-        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, rounds ? nullptr : long_list);
+        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, long_list);
         msm_partition_kernel<Fs><<<sort_ctas, MSM_SORT_THREADS, part_smem, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, P.nb, ts, base_stride,
                                                                                  offsets, rng, parts);
         msm_range_sort_kernel<<<MSM_RSORT_CTAS_PER_SM * sm_count(), MSM_SORT_THREADS, 0, s>>>(offsets, P.nb, parts, cursor, sorted);
@@ -1108,36 +957,12 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
         msm_count_kernel<Fs><<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, counts);
         msm_scan_tile_sums_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_sums);
         msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
-        // the offsets the accumulation walks also give the merge its long buckets (after the last pair round, if any)
-        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, rounds ? nullptr : long_list);
+        // the offsets the accumulation walks also give the merge its long buckets
+        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, offsets, P.seg, long_list);
         msm_scatter_kernel<Fs><<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const Fs *)d_scalars, sub, n, fmt, P.c, P.nwin, key_stride, base_stride, offsets, cursor, sorted);
     }
     if (ctx->profile) LURK_CUDA_TRY(cudaEventRecord(ctx->ev0, s));
-    // ---- pair rounds
-    const uint32_t *acc_offs = offsets;
-    const Affine<Fb> *acc_pts = bases;
-    size_t cap_r = cap;
-    for (int r = 0; r < rounds; r++) {
-        cap_r = cap_r / 2 + TB + 1;                                        // sum of ceil(m_k / 2) <= cap / 2 + buckets
-        DevBuf &ob = S.pair_offs[r & 1], &pb = S.pair_pts[r & 1];
-        if (ob.bytes < ((size_t)TB + 1) * sizeof(uint32_t)) LURK_TRY(ob.alloc(((size_t)TB + 1) * sizeof(uint32_t)));
-        if (pb.bytes < cap_r * sizeof(Affine<Fb>)) LURK_TRY(pb.alloc(cap_r * sizeof(Affine<Fb>)));
-        uint32_t *o2 = ob.as<uint32_t>();
-        msm_halve_kernel<<<(TB + 256) / 256, 256, 0, s>>>(acc_offs, TB, counts);          // `counts` is free after the scatter
-        msm_scan_tile_sums_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_sums);
-        msm_scan_tiles_kernel<<<1, 1024, 0, s>>>(tile_sums, ntiles, tile_offsets);
-        msm_scan_apply_kernel<<<ntiles, 1024, 0, s>>>(counts, TB, tile_offsets, ntiles, o2, P.seg, r == rounds - 1 ? long_list : nullptr);
-        const size_t pthreads = (cap_r + PAIR_B - 1) / PAIR_B;
-        const unsigned pgrid = (unsigned)((pthreads + 127) / 128);
-        if (r == 0) msm_pair_kernel<Fb, true><<<pgrid, 128, 0, s>>>(acc_offs, o2, TB, sorted, acc_pts, pb.as<Affine<Fb>>());
-        else msm_pair_kernel<Fb, false><<<pgrid, 128, 0, s>>>(acc_offs, o2, TB, sorted, acc_pts, pb.as<Affine<Fb>>());
-        launches += 5;
-        acc_offs = o2;
-        acc_pts = pb.as<Affine<Fb>>();
-    }
-    if (rounds)
-        msm_accumulate_kernel<Fb, 5, true><<<(t1 + 127) / 128, 128, 0, s>>>(acc_offs, TB, sorted, acc_pts, buckets, S.ppt.as<Pt>(), P.seg, t1);
-    else if (fixed)
+    if (fixed)
         msm_accumulate_kernel<Fb, 5><<<(P.t1 + 127) / 128, 128, 0, s>>>(offsets, TB, sorted, bases, buckets, S.ppt.as<Pt>(), P.seg, P.t1);
     else
         msm_accumulate_kernel<Fb, 4><<<(P.t1 + 127) / 128, 128, 0, s>>>(offsets, TB, sorted, bases, buckets, S.ppt.as<Pt>(), P.seg, P.t1);
@@ -1145,9 +970,9 @@ int msm_launch(lurk_msm_ctx *ctx, const void *d_scalars, size_t n, int fmt, cuda
     launches += 6;
     // merge of the partials into their buckets: long buckets (one CTA each, a grid of at most two per SM walking the list)
     // and the others (one thread each) are disjoint, so the two launches do not depend on each other
-    msm_merge_long_kernel<Fb><<<std::min<uint32_t>(max_long, 2 * sm_count()), MSM_MERGE_LONG_THREADS, 0, s>>>(acc_offs, P.seg, S.ppt.as<Pt>(),
+    msm_merge_long_kernel<Fb><<<std::min<uint32_t>(max_long, 2 * sm_count()), MSM_MERGE_LONG_THREADS, 0, s>>>(offsets, P.seg, S.ppt.as<Pt>(),
                                                                                                              long_list, buckets);
-    msm_merge_kernel<Fb><<<(TB + MSM_MERGE_THREADS - 1) / MSM_MERGE_THREADS, MSM_MERGE_THREADS, 0, s>>>(acc_offs, TB, P.seg, S.ppt.as<Pt>(), buckets);
+    msm_merge_kernel<Fb><<<(TB + MSM_MERGE_THREADS - 1) / MSM_MERGE_THREADS, MSM_MERGE_THREADS, 0, s>>>(offsets, TB, P.seg, S.ppt.as<Pt>(), buckets);
     launches += 2;
     // bucket reduction: chunk sums, per-bit tree sums, (slice sums); the host finishes with a Horner over nq points per set
     const uint32_t nchunks = P.rwin * P.G, nres = P.rwin * P.nq;

@@ -184,19 +184,3 @@ def test_msm_sizes_around_plan_boundaries(L, oracle, spec, n):
     assert np.array_equal(ck.commit(sc), want)
     m = max(1, n // 3)                                   # a shorter scalar vector on the same (fixed-base) key
     assert np.array_equal(ck.commit(sc[:32 * m]), oracle.msm(curve, bases[:64 * m], sc[:32 * m], nthreads=8, naive=(m < 40)))
-
-
-def test_pair_rounds_path_matches_default_path(tmp_path):
-    """the optional batched-affine pair rounds (LURK_MSM_PAIR_ROUNDS, csrc/msm_impl.cuh: msm_pair_kernel) give the same
-    commitments as the plain XYZZ accumulation: the whole parity file re-run in a subprocess with 2 forced rounds (the switch is
-    read once per process), including the edge cases (doubling inside a bucket, P + (-P), identity bases, single terms)"""
-    import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    if os.environ.get("LURK_MSM_PAIR_ROUNDS"):
-        pytest.skip("already running with forced pair rounds")
-    env = dict(os.environ, LURK_MSM_PAIR_ROUNDS="2")
-    out = subprocess.run([sys.executable, "-m", "pytest", os.path.join(root, "tests", "test_gpu_msm.py"), "-m", "gpu", "-q", "-x",
-                          "-k", "not pair_rounds"], capture_output=True, text=True, timeout=900, cwd=root, env=env)
-    assert out.returncode == 0, out.stdout[-3000:]

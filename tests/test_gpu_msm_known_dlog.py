@@ -15,9 +15,6 @@ happen in the model, so a later plan change cannot quietly stop a test from reac
 asserts that together they reach every named branch of every kernel.
 """
 import functools
-import os
-import subprocess
-import sys
 from collections import Counter
 
 import numpy as np
@@ -85,7 +82,7 @@ def signed_digits(s, c, nwin):
 
 
 class Group:
-    """point additions on discrete logs mod q: each records which branch of XYZZ::add / add_affine / the pair kernel it takes"""
+    """point additions on discrete logs mod q: each records which branch of XYZZ::add / add_affine it takes"""
 
     def __init__(self, q):
         self.q, self.seen = q, set()
@@ -160,7 +157,6 @@ def model(plan, key_dlog, kidx, sval, sidx, q, warp_sort):
             B[key] = total                       # the order inside the bucket is the atomics': only its sum is known
             continue
         facts.add(("bucket", "exact"))
-        _pair_rounds(grp, [at(t) for t in range(min(hi - lo, 64))])
         # pieces of the bucket cut at segment boundaries: the first is the bucket's own slot, the others partials
         memo, pieces, a = {}, [], lo
         while a < hi:
@@ -263,16 +259,6 @@ def _bitsum(grp, plan, tri, runs, w, qq, sl):
     for tid, _, v in sorted(items):
         sm[tid] = grp.add("bitsum", sm[tid], v)
     return _tree(grp, "bitsum", sm)
-
-
-def _pair_rounds(grp, seq):
-    """two rounds of msm_pair_kernel on the start of an exactly known bucket: entries 2j and 2j + 1 are added (kind 2 doubles,
-    kind 3 gives the identity)"""
-    for _ in range(2):
-        out = []
-        for j in range(0, len(seq), 2):
-            out.append(grp.add("pair", seq[j], seq[j + 1]) if j + 1 < len(seq) else seq[j])
-        seq = out
 
 
 # ------------------------------------------------------------------------------------------------------------ degenerate patterns
@@ -386,9 +372,9 @@ def designed(pattern, plan, seen, n_used, warp_sort):
         elif plan.G >= 2:
             want.add(("host", "dbl"))
     elif pattern == "alternating":
-        want |= {("accumulate", "inf"), ("pair", "inf")}
+        want.add(("accumulate", "inf"))
         if plan.n >= 5:
-            want |= {("accumulate", "dbl"), ("pair", "dbl")}
+            want.add(("accumulate", "dbl"))
         if plan.n >= 64:
             want.add(("bucket", "inf"))
     elif pattern == "blocks":
@@ -514,24 +500,11 @@ def test_model_reaches_every_branch(spec):
             for c in FIXED_WINDOWS:
                 for ws in (False, True):
                     seen |= Case(spec, curve, pattern, FIXED_N, c, warp_sort=ws, device=False).seen
-    want = {("accumulate", b) for b in ("dbl", "inf", "id_rhs")} | {("pair", "dbl"), ("pair", "inf")}
+    want = {("accumulate", b) for b in ("dbl", "inf", "id_rhs")}
     want |= {(s, b) for s in ("merge", "merge_long") for b in ("dbl", "inf")}
     want |= {("chunk", "dbl"), ("bitsum", "dbl"), ("slice", "dbl"), ("horner", "dbl"), ("host", "dbl"), ("precompute", "id")}
     want |= {("bucket", "inf"), ("bucket", "long")}
     assert not want - seen, sorted(want - seen)
-
-
-def test_pair_rounds(tmp_path):
-    """the batched-affine pair rounds (msm_pair_kernel: kind 2 doubles, kind 3 gives the identity) on the same degenerate inputs:
-    the file re-run with 1 and 2 forced rounds (the switch is read once per process)"""
-    if os.environ.get("LURK_MSM_PAIR_ROUNDS"):
-        pytest.skip("already running with forced pair rounds")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for rounds in ("1", "2"):
-        env = dict(os.environ, LURK_MSM_PAIR_ROUNDS=rounds)
-        out = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider",
-                              "-k", "degenerate or launch_device"], capture_output=True, text=True, timeout=1800, cwd=root, env=env)
-        assert out.returncode == 0, (rounds, out.stdout[-3000:])
 
 
 # --------------------------------------------------------------------------------------------------------------- distinct-point keys

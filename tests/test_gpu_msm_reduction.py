@@ -102,18 +102,3 @@ def test_reduction_long_buckets_everywhere(L, oracle, spec):
     assert np.array_equal(ck.commit(sc), want)
     ck.precompute()
     assert np.array_equal(ck.commit(sc), want)
-
-
-def test_reduction_with_pair_rounds(tmp_path):
-    """the same distributions with the batched-affine pair rounds forced on (LURK_MSM_PAIR_ROUNDS is read once per process):
-    the accumulation and the merge then walk the offsets of the halved lists"""
-    import os
-    import subprocess
-    import sys
-    if os.environ.get("LURK_MSM_PAIR_ROUNDS"):
-        pytest.skip("already running with forced pair rounds")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, LURK_MSM_PAIR_ROUNDS="2")
-    out = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-m", "gpu", "-q", "-x", "-k",
-                          "distributions or long_buckets"], capture_output=True, text=True, timeout=900, cwd=root, env=env)
-    assert out.returncode == 0, out.stdout[-3000:]
